@@ -2,6 +2,7 @@
 """Benchmark of the Fp frequency-sweep hot path (BASELINE.json metric: Fp evals/s).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload C4|C2|C3|C5] [--impl ours|reference]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Default workload = the configuration the metric is quoted on (BASELINE.json north_star / configs[3]):
@@ -32,6 +33,12 @@ the same bins, bit for bit (every rank recomputes a slice of ANOTHER rank's shar
 spot check of bins of the timed result. `--impl reference` times the CPU restatement of the reference
 (oracle/, NumPy + threaded pieces, all host cores) on a bounded sample of the same workload; together with
 `cpu_baseline` and the spot check it is the only place outside tests/ and smoke() that executes oracle/.
+
+`--dump-outputs DIR` writes what the last timed step of the primary workload returned (rank 0, after the timing)
+as DIR/<name>.npy in float64: `fp.npy`, the (F,) Fp values of a plain sweep, or `nmfp.npy`, the (D, F) values of
+a noise-marginalised one. An output above 64 MB is replaced by a fixed, seeded sample of its rows
+(`nmfp_rows.npy` holds their indices as float64). The inputs are seeded, so two builds run with the same arguments
+can be compared output for output.
 """
 from __future__ import annotations
 
@@ -117,7 +124,7 @@ def measured_peaks():
         with open(path) as f:
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 def config_of(key, wl, gpus):
@@ -139,7 +146,7 @@ def config_of(key, wl, gpus):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (recipe in B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -337,6 +344,8 @@ class Ctx:
             os.environ.setdefault("NCCL_DEBUG", "WARN")  # keep NCCL's version banner off stdout (one JSON line)
             dist.init_process_group("nccl", device_id=self.dev)
         self.flush_buf = torch.empty(256 * 1024 * 1024 // 8, dtype=torch.float64, device=self.dev)
+        self.last = None  # what the last timed step returned
+        self.dump_dir = None  # --dump-outputs: set for the primary workload only
 
     def barrier(self):
         if self.world > 1:
@@ -351,7 +360,7 @@ class Ctx:
         for a, b in ev:
             self.flush_buf.fill_(1.0)  # L2 flush, outside the timed bracket
             a.record()
-            fn()
+            self.last = fn()
             b.record()
         self.barrier()
         t = torch.tensor([sum(a.elapsed_time(b) for a, b in ev)], dtype=torch.float64, device=self.dev)
@@ -368,6 +377,24 @@ class Ctx:
     def close(self):
         if self.world > 1:
             self.dist.destroy_process_group()
+
+
+DUMP_MAX_BYTES = 64 * 2**20
+
+
+def dump_output(ctx, name, out):
+    """--dump-outputs: the last timed step's result as DIR/<name>.npy (float64); a (D, F) result above 64 MB keeps a
+    seeded sample of its rows, whose indices go to DIR/<name>_rows.npy"""
+    if ctx.dump_dir is None or ctx.rank != 0:
+        return
+    os.makedirs(ctx.dump_dir, exist_ok=True)
+    a = out.detach().to("cpu", ctx.torch.float64).numpy()
+    if a.nbytes > DUMP_MAX_BYTES:
+        keep = max(1, DUMP_MAX_BYTES // (2 * a[0].nbytes))
+        rows = np.sort(np.random.default_rng(20240607).choice(a.shape[0], size=keep, replace=False))
+        a = a[rows]
+        np.save(os.path.join(ctx.dump_dir, f"{name}_rows.npy"), rows.astype(np.float64))
+    np.save(os.path.join(ctx.dump_dir, f"{name}.npy"), np.ascontiguousarray(a))
 
 
 def same_bits(torch, a, b):
@@ -442,6 +469,7 @@ def run_fp(key, wl, ctx, steps, warmup, with_cpu_baseline):
     total_ms = ctx.timed(step_device, steps)
     launches = _cabi.kernel_launches() - launches0
     clocks = sampler.stop() if rank == 0 else None
+    dump_output(ctx, "fp", ctx.last)
     ms_step = total_ms / steps
     ne2e = e2e_steps_for(steps, ms_step)
     for _ in range(2 if ms_step < 1000.0 else 1):
@@ -524,7 +552,7 @@ def run_fp(key, wl, ctx, steps, warmup, with_cpu_baseline):
     ach_tf = evals_kernel * flops_per_eval(wl["n"], m_basis) / (kern_ms * 1e-3) / 1e12
     if sweep_path == "i8":
         # The contraction runs on the INT8 tensor path: Y = G [s c] as 28 products of 8-bit digit planes
-        # (tcgen05.mma kind::i8, exact int32 accumulation). Algorithmic integer ops per eval: 28 plane products
+        # (wgmma .s32.s8.s8, exact int32 accumulation). Algorithmic integer ops per eval: 28 plane products
         # x 2 (multiply, add) x 2 columns (sin, cos) x (m + 1) rows (basis + the C^-1 r row) x n TOAs.
         i8_peak, _ = _cabi.fp64_peak(17, 2000, device=ctx.local)
         i8_shape, _ = _cabi.fp64_peak(18, 4000, device=ctx.local)
@@ -533,36 +561,34 @@ def run_fp(key, wl, ctx, steps, warmup, with_cpu_baseline):
         nst = -(-wl["n"] // 32)
         rows_pad = 32 * -(-(m_basis + 1) // 32)
         passes = -(-rows_pad // 128)  # row groups of 128 operand rows: one pass over the TOAs each
-        items = wl["P"] * -(-(hi - lo) // 32) * passes
-        exec_top = items * nst * 28.0 * 2.0 * 128 * 64 * 32 / (kern_ms * 1e-3) / 1e12
-        smem_stage = 28.0 * 6144 + 7.0 * min(rows_pad, 128) * 32 + 14336
+        items = wl["P"] * -(-(hi - lo) // 16) * passes
+        exec_top = items * nst * 28.0 * 2.0 * 128 * 32 * 32 / (kern_ms * 1e-3) / 1e12
+        smem_stage = 28.0 * 2 * 3072 + 7.0 * min(rows_pad, 128) * 32 + 7168
         sm_count = torch.cuda.get_device_properties(ctx.local).multi_processor_count
         smem_peak = 128.0 * sm_count * (clocks["sm_mhz"] if clocks and clocks.get("sm_mhz") else 1965.0) * 1e6 / 1e9
         roofline = {
-            "bound": "tensor", "pipe": "INT8 tensor path (tcgen05.mma kind::i8, int32 accumulators in tensor memory)",
+            "bound": "tensor", "pipe": "INT8 tensor path (wgmma .s32.s8.s8, int32 accumulators in registers)",
             "achieved": ach_top, "peak": i8_peak, "unit": "TOP/s", "frac": ach_top / i8_peak,
             "traffic": traffic, "traffic_source": traffic_src,
-            "peak_source": "measured live on this GPU: fastfp_fp64_peak kind 17 (back-to-back kind::i8 MMAs, M=128 N=256 K=32, "
-                           "one issuing thread per SM); MEASURED_PEAKS.json holds a bf16 figure only",
-            "kernel": "fp_sweep_i8_kernel (persistent, warp-specialised: TMA / MMA issue / epilogue / sincos producers)",
+            "peak_source": "measured live on this GPU: fastfp_fp64_peak kind 17 (back-to-back s8 wgmmas, m64n256k32, "
+                           "two warpgroups per SM); MEASURED_PEAKS.json holds a bf16 figure only",
+            "kernel": "fp_sweep_i8_kernel (persistent, warp-specialised: TMA / wgmma issue + epilogue / sincos producers)",
             "kernel_ms": kern_ms, "ops_per_eval": ops_eval,
             "shape_bound": {"achieved": exec_top, "peak": i8_shape, "unit": "TOP/s", "frac": exec_top / i8_shape,
                             "note": "executed MMA work (128-row operands, m + 1 real rows in all) against the "
-                                    "same 28-product stage issued back to back (kind 18): an M=128 N=64 K=32 MMA reads 6 KB "
-                                    "of operands from shared memory = 48 cycles at 128 B/clk, against 32 cycles of tensor "
-                                    "time -- shared-memory operand bandwidth is what binds this formulation (TMEM holds "
-                                    "7 accumulators x 64 columns, so N cannot grow)"},
+                                    "same 28-product stage issued back to back (kind 18): each m64n32k32 wgmma reads 3 KB "
+                                    "of operands from shared memory; the 7 accumulators of a 128 x 32 tile take 112 "
+                                    "registers per consumer thread, so N cannot grow"},
             "smem_bound": {
                 "achieved": items * nst * smem_stage / (kern_ms * 1e-3) / 1e9, "peak": smem_peak, "unit": "GB/s",
                 "frac": items * nst * smem_stage / (kern_ms * 1e-3) / 1e9 / smem_peak, "bytes_per_stage": smem_stage,
-                "note": "shared-memory traffic of one 32-TOA x 32-frequency stage (28 MMAs x 6 KB of operand reads, the TMA "
-                        "write of the G planes, the producers' 14 KB of sin/cos planes) against 128 B/clk/SM at the sampled "
-                        "SM clock: the floor of this formulation; the rest of the step is the fp64 sin/cos work, which "
-                        "shares a resource with the MMAs on the SM (DESIGN.md 4b)"},
+                "note": "shared-memory traffic of one 32-TOA x 16-frequency stage (2 x 28 wgmmas x 3 KB of operand reads, "
+                        "the TMA write of the G planes, the producers' 7 KB of sin/cos planes) against 128 B/clk/SM at the "
+                        "sampled SM clock: the floor of this formulation; the rest of the step is the fp64 sin/cos work"},
             "fp64_equivalent": {"achieved": ach_tf, "unit": "TFLOP/s", "fp64_pipe_peak": fp64_peak,
                                 "ratio": ach_tf / fp64_peak,
                                 "note": "the same statistic in fp64 flops (4m+10)n per eval against the fp64 pipe peak the "
-                                        "DMMA kernel is bound by (round 1: 0.68): above 1 because the contraction left that pipe"},
+                                        "DMMA kernel is bound by"},
             "note": "algorithmic INT8 ops = 112 (m+1) n per eval; padding rows of the 128-row operand and the producers' "
                     "fp64 sincos work are not counted"}
     else:
@@ -585,7 +611,7 @@ def run_fp(key, wl, ctx, steps, warmup, with_cpu_baseline):
                 "l2": "256 MiB buffer written between timed steps (L2 flush); packed inputs are "
                       f"{pack_bytes / 2**20:.0f} MiB per GPU",
                 "pack_ms_one_time": pack_ms, "content_hash_ms_per_call": hash_ms,
-                "sweep_kernel": {"i8": "INT8 tensor-core kernel (tcgen05 / TMEM)", "fp64": "fp64 DMMA kernel"}[sweep_path],
+                "sweep_kernel": {"i8": "INT8 tensor-core kernel (wgmma)", "fp64": "fp64 DMMA kernel"}[sweep_path],
                 "freqs_total": F_total, "evals_per_step": evals_step},
         "e2e": {"value": evals_step / e2e_ms * 1e3, "unit": "evals/s", "ms_per_step": e2e_ms, "steps": ne2e,
                 "h2d_bytes_per_step": int(8 * F_total), "d2h_bytes_per_step": int(8 * F_total * world),
@@ -656,6 +682,7 @@ def run_nmfp(key, wl, ctx, steps, warmup, with_cpu_baseline):
     total_ms = ctx.timed(step_device, steps)
     launches = _cabi.kernel_launches() - launches0
     clocks = sampler.stop() if rank == 0 else None
+    dump_output(ctx, "nmfp", ctx.last)
     ms_step = total_ms / steps
     ne2e = e2e_steps_for(steps, ms_step)
     for _ in range(2 if ms_step < 1000.0 else 1):
@@ -795,7 +822,9 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-secondary", action="store_true")
     ap.add_argument("--sweep-path", choices=["auto", "fp64", "i8", "prefer-i8"], default=None,
-                    help="kernel of the plain-Fp sweep (default auto: the INT8 tensor-core kernel when the pack fits it)")
+                    help="kernel of the plain-Fp sweep (default auto: the fp64 DMMA kernel)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's output of the primary workload to DIR/<name>.npy (float64)")
     args = ap.parse_args()
     if args.steps < 1:
         raise SystemExit("--steps must be >= 1")
@@ -817,7 +846,9 @@ def main():
         os.environ["FASTFP_B200_PATH"] = args.sweep_path
     ctx = Ctx(rank, world, local)
     runner = run_nmfp if wl["kind"] == "nmfp" else run_fp
+    ctx.dump_dir = args.dump_outputs
     line = runner(key, wl, ctx, args.steps, args.warmup, not args.no_cpu_baseline)
+    ctx.dump_dir = None
     if args.workload is None and not args.no_secondary:
         sec = {}
         for k2 in ("C2", "C3", "W"):
@@ -834,7 +865,7 @@ def main():
             bad += [f"{k2}.{name}" for name, c in l2.get("checks", {}).items() if c.get("ok") is False]
         line["checks_failed"] = bad
         # tuning switches of the library that change the schedule, never the results: recorded when set
-        knobs = {k: os.environ[k] for k in ("FASTFP_B200_PATH", "FASTFP_B200_I8_NPW", "FASTFP_B200_NMFP_LF_MB")
+        knobs = {k: os.environ[k] for k in ("FASTFP_B200_PATH", "FASTFP_B200_NMFP_LF_MB")
                  if k in os.environ}
         if knobs:
             line["env"] = knobs

@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""Fp-statistic frequency scan with the B200 engine: the counterpart of the reference's
+"""Fp-statistic frequency scan with the fastfp_b200 engine: the counterpart of the reference's
 ``examples/run_fp.py`` (same flow, same output file: a JSON dictionary ``{frequency: Fp}``).
 
 Two ways to get the inputs:

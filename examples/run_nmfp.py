@@ -1,5 +1,5 @@
 # -*- coding: utf-8 -*-
-"""Noise-marginalised Fp with the B200 engine: the counterpart of the reference's ``examples/run_nmfp.py``
+"""Noise-marginalised Fp with the fastfp_b200 engine: the counterpart of the reference's ``examples/run_nmfp.py``
 (same flow and flags; output ``res/<savefile>.npy`` holding the ``(nsamples, ncwfreqs)`` array, draw-major).
 
 Two ways to get the inputs:

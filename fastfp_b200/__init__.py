@@ -1,8 +1,8 @@
-"""fastfp_b200 -- a B200-native engine for the pulsar-timing Fp-statistic frequency scan.
+"""fastfp_b200 -- an H100-native engine for the pulsar-timing Fp-statistic frequency scan.
 
 Drop-in for the hot path of gabefreedman/fastfp (``FastFp.calculate_Fp``, ``NMFP.calculate_nmfp``,
 ``fastfp.utils.get_xCy``): same Python call signatures, with the JAX/XLA kernels replaced by
-hand-written fp64 CUDA kernels for sm_100a behind a C ABI (``include/fastfp_b200.h``).
+hand-written fp64 CUDA kernels for sm_90a behind a C ABI (``include/fastfp_b200.h``).
 """
 from .blockn import BlockNvec
 from .fastfp import FastFp

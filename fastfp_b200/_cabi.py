@@ -129,7 +129,7 @@ def check(rc: int) -> None:
 def require_device() -> int:
     n = load().fastfp_device_count()
     if n < 1:
-        raise FastFpError("no CUDA device visible: the Fp hot path only runs on a B200 (no CPU fallback)")
+        raise FastFpError("no CUDA device visible: the Fp hot path only runs on an H100 (no CPU fallback)")
     return n
 
 
@@ -204,12 +204,12 @@ class Pack:
         self.n, self.m = list(n), list(m)
         self._warn_if_not_spd()
 
-    PATHS = {"auto": 0, "fp64": 1, "i8": 2}
+    PATHS = {"auto": 0, "fp64": 1, "i8": 2, "mixed": 3}
 
     def set_path(self, path: str) -> None:
-        """Kernel of the plain-Fp sweep: "auto" (default: the INT8 tensor-core kernel when the pack has digit
-        planes), "fp64" (the DMMA kernel) or "i8" (raises unless every pulsar fits); ``path`` then
-        reads "fp64", "i8" or "mixed" (auto, with the pulsars the tensor kernel does not take on the fp64 kernel)."""
+        """Kernel of the plain-Fp sweep: "auto" (default: the fp64 DMMA kernel), "fp64", "i8" (the INT8
+        tensor-core kernel; raises unless every pulsar fits) or "mixed" (the tensor kernel for the pulsars it takes,
+        the fp64 kernel for the others; raises if it takes none); ``path`` then reads "fp64", "i8" or "mixed"."""
         check(load().fastfp_pack_set_path(self._h, self.PATHS[path]))
 
     @property

@@ -1,4 +1,4 @@
-"""Build libfastfp_b200.so in-tree with nvcc for sm_100a (no torch, no cmake).
+"""Build libfastfp_b200.so in-tree with nvcc for sm_90a (H100) (no torch, no cmake).
 
 ``python -m fastfp_b200.build`` or ``__graft_entry__.build()``. nvcc cross-compiles without a
 GPU. The library links cudart statically, so it only needs the driver at run time.
@@ -19,7 +19,7 @@ OUT_DIR = os.path.join(HERE, "_lib")
 LIB = os.path.join(OUT_DIR, "libfastfp_b200.so")
 SOURCES = ["cabi.cu", "precompute.cu", "fp_sweep.cu", "fp_sweep_w1.cu", "fp_sweep_w2.cu", "fp_sweep_w4.cu",
            "fp_sweep_wide.cu", "fp_sweep_xwide.cu", "fp_sweep_i8.cu", "fe.cu", "nmfp.cu", "xcy.cu", "microbench.cu", "hostutil.cu"]
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-fmad=true"]
 # developer builds only (e.g. FASTFP_B200_NVCC_FLAGS=-DFFP_DEBUG_SWITCHES for tools/dbg_split.sh); the
 # shipped library is built without it and bench.py refuses to run a library built with extra flags

@@ -48,7 +48,7 @@ def draws_from_chain(chain, param_names: Sequence[str], nsamples: int, burn_frac
 
 def draw_batches(samples: Dict[str, np.ndarray], batch_size: int):
     """The draw-batch loop of the reference (``run_nmfp.py:256-270``) as a generator of sub-dicts; the
-    B200 engine batches draws internally, so this is only needed to bound the ``(D, F)`` output."""
+    engine batches draws internally, so this is only needed to bound the ``(D, F)`` output."""
     D = len(next(iter(samples.values())))
     for start in range(0, D, batch_size):
         yield {k: v[start:start + batch_size] for k, v in samples.items()}

@@ -222,13 +222,17 @@ int fastfp_pack_create(int device, int P, const int64_t* n, const int64_t* m,
 }
 
 int fastfp_pack_set_path(fastfp_pack_t* pk, int path) {
-  if (!pk || path < FASTFP_PATH_AUTO || path > FASTFP_PATH_I8) {
+  if (!pk || path < FASTFP_PATH_AUTO || path > FASTFP_PATH_MIXED) {
     set_error("fastfp_pack_set_path: invalid argument");
     return FASTFP_ERR_INVALID;
   }
   if (path == FASTFP_PATH_I8 && !(pk->i8_ok && pk->i8_all())) {
     set_error("fastfp_pack_set_path: not every pulsar of this pack has INT8 digit planes (block-diagonal N, m > 639, "
-              "n > 16384 or non-finite data); FASTFP_PATH_AUTO sweeps those on the fp64 kernel");
+              "n > 16384 or non-finite data); FASTFP_PATH_MIXED sweeps those on the fp64 kernel");
+    return FASTFP_ERR_UNSUPPORTED;
+  }
+  if (path == FASTFP_PATH_MIXED && !pk->i8_ok) {
+    set_error("fastfp_pack_set_path: no pulsar of this pack has INT8 digit planes");
     return FASTFP_ERR_UNSUPPORTED;
   }
   pk->path = path;

@@ -1,5 +1,5 @@
 // Internal declarations shared by the CUDA translation units of libfastfp_b200.so.
-// sm_100a only (built with -gencode arch=compute_100a,code=sm_100a).
+// sm_90a only (built with -gencode arch=compute_90a,code=sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -144,11 +144,10 @@ struct fastfp_pack {
   bool i8_ok = false;             // the planes exist (every pulsar fits the tile, all values finite)
   int i8_rows_max = 0;
   int64_t i8_bytes = 0;
-  int path = 0;                   // FASTFP_PATH_AUTO / _FP64 / _I8 (fastfp_pack_set_path)
-  // AUTO resolves to the tensor path wherever the pack can take it (it passed the GPU parity suite on hardware and is
-  // the faster kernel: profiles/README.md); FASTFP_PATH_FP64 forces the DMMA kernel
-  static constexpr bool kAutoPrefersI8 = true;
-  bool use_i8() const { return i8_ok && (path == 2 || (path == 0 && kAutoPrefersI8)); }
+  int path = 0;                   // FASTFP_PATH_AUTO / _FP64 / _I8 / _MIXED (fastfp_pack_set_path)
+  // AUTO resolves to the fp64 DMMA kernel: on an H100 it sweeps m = 72 bases about twice as fast as the tensor kernel
+  // (C2: 35 ms against 78 ms per step, 400 W H100 SXM). I8 and MIXED select the tensor kernel.
+  bool use_i8() const { return i8_ok && (path == 2 || path == 3); }
   bool i8_all() const { return i8_count == P; }
   int64_t bytes = 0;
   int64_t mvar_total = 0;
@@ -296,6 +295,25 @@ __device__ __forceinline__ void fence_barrier_init() {
 }
 __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+
+// One pulsar's term 0.5 N^T M^-1 N with M = [[m00, m01], [m01, m11]], N = [n0, n1], by LU with partial pivoting like
+// jnp.linalg.solve (fastfp.py:90, nmfp.py:117). Where M is singular to the last bit (the Earth-term basis lies inside
+// span(T), e.g. at f = 1/yr against fitted yearly sinusoids) a pivot is exactly zero; the unknown it would divide out is
+// set to zero (the basic solution) so the term stays finite instead of 0/0. NaN inputs still give NaN.
+__device__ __forceinline__ double term_2x2(double m00, double m01, double m11, double n0, double n1) {
+  const double N0 = n0, N1 = n1;
+  double m10 = m01;
+  if (fabs(m10) > fabs(m00)) {  // row swap; the unknowns keep their order
+    double t0 = m00; m00 = m10; m10 = t0;
+    t0 = m01; m01 = m11; m11 = t0;
+    t0 = n0; n0 = n1; n1 = t0;
+  }
+  const double lq = m00 != 0.0 ? m10 / m00 : 0.0;
+  const double u = m11 - lq * m01;
+  const double x1 = u != 0.0 ? (n1 - lq * n0) / u : 0.0;
+  const double x0 = m00 != 0.0 ? (n0 - m01 * x1) / m00 : 0.0;
+  return 0.5 * (N0 * x0 + N1 * x1);
 }
 
 }  // namespace ffp

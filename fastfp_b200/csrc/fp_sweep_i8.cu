@@ -1,12 +1,12 @@
-// The frequency-sweep kernel on the 5th-generation tensor cores: Y = G [s c] as an error-free product of 8-bit
-// digit planes (tcgen05.mma kind::i8, exact int32 accumulation in tensor memory), everything else in fp64.
+// The frequency-sweep kernel on the INT8 tensor cores: Y = G [s c] as an error-free product of 8-bit digit planes
+// (Hopper wgmma.mma_async .s32.s8.s8, exact int32 accumulation in registers), everything else in fp64.
 //
 // Replaces the body of FastFp.calculate_Fp under jax.vmap (reference fastfp/fastfp.py:69-92, examples/run_fp.py:63)
 // like fp_sweep_kernel.cuh does, for packs with n <= 16384 TOAs per pulsar, a diagonal N and up to 639 basis columns
 // (128 operand rows -- 127 columns + the C^-1 r row -- per pass over the TOAs; wider bases take one pass per row group
-// of 128, the b-sums adding up in the epilogue); the fp64 DMMA kernel stays as the path for everything else. Why: fp64 has no tcgen05 kind, and the DMMA
-// formulation is pinned at 0.68 of the fp64 pipe it has to share with the sincos generation (DESIGN.md section 4.6).
-// The INT8 tensor path is a different unit altogether, and integer accumulation is exact.
+// of 128, the b-sums adding up in the epilogue); the fp64 DMMA kernel stays as the path for everything else. fp64 has
+// no wgmma kind, and the DMMA formulation shares the fp64 pipe with the sincos generation (DESIGN.md section 4.6); the
+// INT8 tensor path is a different unit altogether, and integer accumulation is exact.
 //
 // Number format (radix 256, 7 planes per operand, validated at the level of the statistic by
 // tests/test_split_precision_emulation.py):
@@ -17,19 +17,19 @@
 //   Y_j = 2^(e_j - 13) sum_{g=0..6} 256^-g  sum_{i+j=g} sum_k d_i(k) v_j(k):   28 plane products, one int32
 //        accumulator per weight g (|d v| <= 2^14, 7 products per TOA: exact for n <= 18 724 TOAs)
 //
-// One 768-thread CTA per SM, static round-robin over (pulsar, 32-frequency tile) work items, per stage of 32 TOAs:
-//   warp 0   lane 0: TMA -- one bulk copy of the stage's G planes (7 x rows x 32 bytes, already in the SWIZZLE_32B
-//            K-major operand layout) and one of its (t, 1/N) vectors, mbarrier rings
-//   warps 1-3 lane 0: 28 tcgen05.mma (M = 128: rows of G, N = 64: 32 frequencies x {sin, cos}, K = 32 TOAs) into the
-//            7 accumulators (7 x 64 = 448 of the 512 TMEM columns), split by accumulator over three issuing threads;
-//            tcgen05.commit frees the stage
-//   warps 8-23 (producers, two groups alternating stages): sincos_cw of ((2 pi) f) t (fastfp.py:78-79 phase order),
+// One 640-thread CTA per SM, static round-robin over (pulsar, 16-frequency tile) work items, per stage of 32 TOAs:
+//   warpgroup 0, warp 0 lane 0: TMA -- one bulk copy of the stage's G planes (7 x rows x 32 bytes, already in the
+//            SWIZZLE_32B K-major operand layout) and one of its (t, 1/N) vectors, mbarrier rings
+//   warpgroups 1-2 (consumers, operand rows 0-63 and 64-127 of the row group): 28 wgmma m64n32k32 (N = 32: 16
+//            frequencies x {sin, cos}, K = 32 TOAs) into the 7 register accumulators (7 x 16 registers per thread);
+//            after the last stage of a pass the same warpgroup runs the epilogue: fp64 recombination,
+//            b = Y_s.Y_s, Y_s.Y_c, Y_c.Y_c over the basis rows, (s|r), (c|r) from the w row, pivoted 2x2 solve
+//            (jnp.linalg.solve at fastfp.py:90)
+//   warpgroups 3-4 (producers, one per stage, alternating): sincos_cw of ((2 pi) f) t (fastfp.py:78-79 phase order),
 //            the digit split, 14 conflict-free 4-byte stores per thread into the B-operand planes, and the fp64
 //            sums s N^-1 s, s N^-1 c (c N^-1 c = sum 1/N - s N^-1 s)
-//   warps 4-7 (epilogue, one TMEM lane quarter each): tcgen05.ld, fp64 recombination, b = Y_s.Y_s, Y_s.Y_c, Y_c.Y_c
-//            over the basis rows, (s|r), (c|r) from the w row, pivoted 2x2 solve (jnp.linalg.solve at fastfp.py:90)
-// Shared memory is the bound: an M=128, N=64 MMA reads 6 KB of operands, 48 cycles at 128 B/clk (measured,
-// tools/probes/umma_i8_shape_probe.cu), i.e. 1344 cycles per stage against ~3490 for the same work on the DMMA path.
+// The accumulators of a 128 x 32 tile fill 112 registers of each of the 256 consumer threads, which is what sets the
+// tile at 16 frequencies: 32 would need the whole register file.
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -44,26 +44,22 @@ namespace i8 {
 
 constexpr int NPL = 7;                 // digit planes per operand
 constexpr int KT = 32;                 // TOAs per stage = K bytes per operand row (one SWIZZLE_32B atom wide)
-constexpr int NF = 32;                 // frequencies per work item
-constexpr int NBR = 2 * NF;            // rows of the B operand: row = 32 * {0: sin, 1: cos} + frequency
-constexpr int S_PLANE = NBR * KT;      // 2048 bytes
-constexpr int S_STAGE = NPL * S_PLANE; // 14336 bytes
+constexpr int NF = 16;                 // frequencies per work item
+constexpr int NBR = 2 * NF;            // rows of the B operand: row = 16 * {0: sin, 1: cos} + frequency
+constexpr int S_PLANE = NBR * KT;      // 1024 bytes
+constexpr int S_STAGE = NPL * S_PLANE; // 7168 bytes
 constexpr int V_STAGE = KT * 16;       // (t, 1/N) per TOA
-constexpr int SST = 6, VST = 8;        // ring depths (even: a slot is always served by the same producer group)
+constexpr int SST = 8, VST = 8;        // ring depths (even: a slot is always served by the same producer group)
 constexpr int RS = 640;                // row-scale stride per pulsar: up to 5 row groups of 128 operand rows (m <= 639)
-constexpr int NISSUE = 3;               // MMA-issuing threads (control warps 1-3), each owning a set of accumulators
-// Warp layout: warps 0-3 control (TMA, MMA issue), 4-7 epilogue, 8.. producers. A stage is always produced by 8
-// warps (thread = one frequency x four TOAs); with NPW = 16 two groups of 8 alternate stages, with NPW = 8 one group
-// takes every stage and each producer thread gets twice the registers.
-template <int NPW>
-struct Roles {
-  static_assert(NPW == 8 || NPW == 16, "8 or 16 producer warps");
-  static constexpr int THREADS = 256 + 32 * NPW;
-  static constexpr int NG = NPW / 8;                                   // producer groups
-  static constexpr int REGS_LAUNCH = NPW == 16 ? 80 : 128;             // 65536 / THREADS, multiple of 8
-  static constexpr int REGS_CTRL = 56, REGS_EPI = 136, REGS_PROD = NPW == 16 ? 72 : 152;
-  static_assert(128 * REGS_CTRL + 128 * REGS_EPI + 32 * NPW * REGS_PROD <= THREADS * REGS_LAUNCH, "register pool");
-};
+constexpr int NCONS = 2;               // consumer warpgroups (64 operand rows each)
+constexpr int NACC = 16;               // accumulator registers per thread per weight: 64 x 32 / 128
+// Warp layout: warpgroup 0 control (TMA), 1-2 consumers, 3-4 producers (one group of 4 warps per stage, thread = one
+// frequency x four TOAs, the two groups alternating stages). setmaxnreg moves registers between the warpgroups.
+constexpr int THREADS = 640;
+constexpr int NPW = 8;                 // producer warps
+constexpr int REGS_LAUNCH = 96;        // 65536 / THREADS, multiple of 8
+constexpr int REGS_CTRL = 32, REGS_CONS = 152, REGS_PROD = 72;
+static_assert(128 * REGS_CTRL + 256 * REGS_CONS + 32 * NPW * REGS_PROD <= THREADS * REGS_LAUNCH, "register pool");
 static_assert(SST % 2 == 0 && VST % 2 == 0, "ring depths must be even");
 
 struct Args {
@@ -78,18 +74,10 @@ struct Args {
   double* Z;                     // nmfp stage A: [P][ceil(F/32)][mvpad/4][8][32] z'_s, z'_c tiles (B-fragment order)
   double* A;                     // nmfp stage A: [P][ceil(F/32)][5][32] a_ss, a_sc, a_cc, a_sr, a_cr
   int mvpad;
-  int ntile, nwork;
+  int ntile, nwork;              // 16-frequency tiles per pulsar, work items
+  int nt32;                      // 32-frequency tiles of the nmfp outputs
   int gslot, gst;                // G ring: bytes per slot (7 x rows_max x 32), number of slots
-#ifdef FFP_I8_TRACE
-  long long* trace;              // [TRACE_EV][TRACE_K] clock64 of CTA 0's first stages (tools/i8_trace.py)
-#endif
 };
-#ifdef FFP_I8_TRACE
-constexpr int TRACE_EV = 8, TRACE_K = 512;
-#define FFP_TRACE(ev, k) do { if (ar.trace && blockIdx.x == 0 && (k) < (uint32_t)TRACE_K) ar.trace[(ev) * TRACE_K + (k)] = clock64(); } while (0)
-#else
-#define FFP_TRACE(ev, k) do { } while (0)
-#endif
 
 // byte offset of (row r, K byte c) in a K-major tile with 32-byte rows, SWIZZLE_32B: 8-row groups of 256 bytes, the
 // 16-byte chunk index XORed with bit 2 of the row (validated by tools/probes/umma_i8_split_check.cu)
@@ -188,30 +176,26 @@ __global__ void i8_planes_kernel(const double* __restrict__ packets, const Pulsa
   }
 }
 
+
 // ---- device helpers ------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
-  // K-major, SWIZZLE_32B (layout type 6), stride between 8-row groups 256 bytes, descriptor version 1
-  return (uint64_t)((saddr >> 4) & 0x3fff) | ((uint64_t)1 << 16) | ((uint64_t)(256 >> 4) << 32) | ((uint64_t)1 << 46) |
-         ((uint64_t)6 << 61);
-}
-__device__ __forceinline__ void umma_i8(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
+// wgmma shared-memory descriptor: K-major, SWIZZLE_32B (layout type 3), stride between 8-row groups 256 bytes; the
+// leading-byte offset is unused for swizzled K-major operands one atom wide. Operand bases are 1024-byte aligned.
+constexpr uint64_t DESC_HI = ((uint64_t)(256 >> 4) << 32) | ((uint64_t)3 << 62);
+__device__ __forceinline__ uint32_t desc_lo(uint32_t saddr) { return ((saddr >> 4) & 0x3fffu) | (1u << 16); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
+// D (64 x 32, s32) = A (64 x 32 s8, K-major) B^T (32 x 32 s8, K-major) + (accumulate ? D : 0)
+__device__ __forceinline__ void wgmma_i8(uint32_t (&d)[NACC], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k32.s32.s8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+        "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+      : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.b64 [%0];\n" ::"l"((uint64_t)smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t* v) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];\n"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-               : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 template <int R>
 __device__ __forceinline__ void reg_set_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int R>
@@ -220,8 +204,8 @@ __device__ __forceinline__ void reg_set_dec() { asm volatile("setmaxnreg.dec.syn
 // x in [-1, 1] -> the 7 bytes of Q + 0x80..80, Q = rint(x 2^54), every byte XORed with 0x80: balanced signed digits,
 // most significant in byte 6. The scaling is an integer add on the exponent field (zero and subnormals land below
 // 2^-900 and round to 0; the fast path is entered for finite data only) and the rounding ONE conversion instruction
-// (F2I.S64.F64): conversions keep their rate while tcgen05 MMAs are in flight, fp64 multiplies and FMAs do not
-// (tools/probes/umma_fp64_overlap_probe.cu), and an all-integer extraction costs ~30 instructions per value.
+// (F2I.S64.F64), which keeps the producers off the fp64 pipe for this part; an all-integer extraction costs ~30
+// instructions per value.
 __device__ __forceinline__ uint2 digits7(double x) {
   const long long Q = __double2ll_rn(__hiloint2double(__double2hiint(x) + (54 << 20), __double2loint(x)));
   const long long U = Q + 0x0080808080808080LL;
@@ -236,8 +220,7 @@ __device__ __forceinline__ void wait_timeout(int tag, uint32_t k) {
   __trap();
 }
 // mbarrier.try_wait with a suspend-time hint: the warp sleeps in hardware until the phase completes or HINT_NS pass
-// (without the hint the time slice is a few tens of nanoseconds, and __nanosleep between polls was measured not to
-// lengthen it: the four epilogue warps alone executed a quarter of the kernel's instructions polling for their item).
+// (without the hint the time slice is a few tens of nanoseconds, so waiting warps would spend issue slots polling).
 __device__ __forceinline__ bool mbar_try_wait_hint(uint64_t* bar, uint32_t parity, uint32_t hint_ns) {
   uint32_t ok;
   asm volatile(
@@ -270,92 +253,66 @@ __device__ __forceinline__ void wait_wd(uint64_t* bar, uint32_t parity, int tag,
     }
   }
 }
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}\n" : "=r"(pred));
-  return pred != 0;
-}
 
-// The products of one 32-TOA stage that issuer Q owns: accumulator g = i + j collects plane i of G times plane j of
-// [s c]; the accumulators are dealt to the three issuers as {6, 1}, {5, 2}, {4, 3, 0} (9 + 9 + 10 products). Descriptors
-// differ in their 14-bit address field only, so each is one add on the low word of the stage's base descriptor.
-template <int Q>
-__device__ __forceinline__ void issue_stage(uint32_t tm, uint32_t da_lo, uint32_t db_lo, uint32_t aplane16,
-                                            uint32_t idesc, bool first_stage) {
-  constexpr uint32_t OWNER[NPL] = {2, 0, 1, 2, 2, 1, 0};
-  constexpr uint64_t HI = ((uint64_t)(256 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)6 << 61);
+// The 28 products of one 32-TOA stage for one consumer warpgroup: accumulator g = i + j collects plane i of G times
+// plane j of [s c]; the first product into accumulator g of a pass is (0, g). Descriptors differ in their address
+// field only, so each is one add on the low word of the stage's base descriptor.
+__device__ __forceinline__ void issue_stage(uint32_t (&acc)[NPL][NACC], uint32_t da_lo, uint32_t db_lo,
+                                            uint32_t aplane16, bool first_stage) {
 #pragma unroll
   for (int i = 0; i < NPL; ++i) {
 #pragma unroll
-    for (int j = 0; j < NPL - i; ++j) {  // the first product into accumulator j of an item is (0, j)
-      if (OWNER[i + j] == (uint32_t)Q)
-        umma_i8(tm + (uint32_t)((i + j) * NBR), HI | (uint64_t)(da_lo + (uint32_t)i * aplane16),
-                HI | (uint64_t)(db_lo + (uint32_t)j * (S_PLANE >> 4)), idesc, (!first_stage || i > 0) ? 1u : 0u);
-    }
+    for (int j = 0; j < NPL - i; ++j)
+      wgmma_i8(acc[i + j], DESC_HI | (uint64_t)(da_lo + (uint32_t)i * aplane16),
+               DESC_HI | (uint64_t)(db_lo + (uint32_t)j * (S_PLANE >> 4)), (!first_stage || i > 0) ? 1u : 0u);
   }
 }
 
 struct Smem {
   unsigned char *G, *S, *V;
-  double *redA;          // [2][2][NF][3] producer sums: buffer, producer group (one or two), frequency
-  double *part;          // [4][NF][3]    epilogue partial b-sums per warp
+  double *redA;          // [2][2][NF][3] producer sums: buffer, producer group, frequency
+  double *part;          // [8][NF][3]    epilogue partial b-sums per consumer warp
   double *nval;          // [NF][2]       (s|r), (c|r) from the w row
-  uint64_t *g_full, *g_empty, *v_full, *v_empty, *s_full, *s_empty, *acc_full, *acc_empty, *sums_full, *sums_empty;
-  uint32_t* tmem;
+  uint64_t *g_full, *g_empty, *v_full, *v_empty, *s_full, *s_empty, *sums_full, *sums_empty;
   __device__ Smem(unsigned char* raw, const Args& ar) {
     G = raw;
     S = G + (size_t)ar.gst * ar.gslot;
     V = S + SST * S_STAGE;
     redA = reinterpret_cast<double*>(V + VST * V_STAGE);
     part = redA + 2 * 2 * NF * 3;
-    nval = part + 4 * NF * 3;
+    nval = part + 8 * NF * 3;
     g_full = reinterpret_cast<uint64_t*>(nval + NF * 2);
     g_empty = g_full + 8;
     v_full = g_empty + 8;
     v_empty = v_full + VST;
     s_full = v_empty + VST;
     s_empty = s_full + SST;
-    acc_full = s_empty + SST;
-    acc_empty = acc_full + 1;
-    sums_full = acc_empty + 1;
+    sums_full = s_empty + SST;
     sums_empty = sums_full + 2;
-    tmem = reinterpret_cast<uint32_t*>(sums_empty + 2);
   }
 };
-constexpr size_t SMEM_FIXED = (size_t)SST * S_STAGE + VST * V_STAGE + (2 * 2 * NF * 3 + 4 * NF * 3 + NF * 2) * 8 +
-                              (8 + 8 + 2 * VST + 2 * SST + 2 + 4) * 8 + 16;
+constexpr size_t SMEM_FIXED = (size_t)SST * S_STAGE + VST * V_STAGE + (2 * 2 * NF * 3 + 8 * NF * 3 + NF * 2) * 8 +
+                              (8 + 8 + 2 * VST + 2 * SST + 4) * 8;
 
-template <bool NMFP, int NPW>
-__global__ void __launch_bounds__(Roles<NPW>::THREADS, 1) fp_sweep_i8_kernel(const Args ar) {
-  using R = Roles<NPW>;
-  constexpr int NG = R::NG;
+template <bool NMFP>
+__global__ void __launch_bounds__(THREADS, 1) fp_sweep_i8_kernel(const Args ar) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   Smem sm(smem_raw, ar);
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   if (tid == 0) {
-    for (int s = 0; s < ar.gst; ++s) { mbar_init(&sm.g_full[s], 1); mbar_init(&sm.g_empty[s], NISSUE); }
-    for (int s = 0; s < VST; ++s) { mbar_init(&sm.v_full[s], 1); mbar_init(&sm.v_empty[s], 8); }
-    for (int s = 0; s < SST; ++s) { mbar_init(&sm.s_full[s], 8); mbar_init(&sm.s_empty[s], NISSUE); }
-    mbar_init(sm.acc_full, NISSUE);
-    mbar_init(sm.acc_empty, 4);
+    for (int s = 0; s < ar.gst; ++s) { mbar_init(&sm.g_full[s], 1); mbar_init(&sm.g_empty[s], NCONS); }
+    for (int s = 0; s < VST; ++s) { mbar_init(&sm.v_full[s], 1); mbar_init(&sm.v_empty[s], 4); }
+    for (int s = 0; s < SST; ++s) { mbar_init(&sm.s_full[s], 4); mbar_init(&sm.s_empty[s], NCONS); }
     for (int b = 0; b < 2; ++b) { mbar_init(&sm.sums_full[b], NPW); mbar_init(&sm.sums_empty[b], 1); }
     fence_barrier_init();
   }
-  if (wid == 1) {  // the MMA warp owns the tensor-memory allocation (all 512 columns: one CTA per SM)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(sm.tmem)), "n"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tm = *sm.tmem;
 
   if (wid < 4) {
-    // ================= control warpgroup: TMA (warp 0) and MMA issue (warp 1) =================
-    reg_set_dec<R::REGS_CTRL>();
+    // ================= control warpgroup: TMA (warp 0, lane 0) =================
+    reg_set_dec<REGS_CTRL>();
     if (wid == 0 && lane == 0) {
-      // ring positions and phase parities are carried incrementally (a division by the runtime ring depth per stage
-      // costs ~25 dependent instructions on a thread that competes with 16 producer warps for issue slots)
+      // ring positions and phase parities are carried incrementally (no division by the runtime ring depth per stage)
       uint32_t k = 0, sv = 0, vpar = 0, sg = 0, gpar = 0;
       unsigned char* gdst = sm.G;
       for (int item = blockIdx.x; item < ar.nwork; item += gridDim.x) {
@@ -372,7 +329,6 @@ __global__ void __launch_bounds__(Roles<NPW>::THREADS, 1) fp_sweep_i8_kernel(con
             mbar_expect_tx(&sm.v_full[sv], V_STAGE);
             tma_load_1d(sm.V + sv * V_STAGE, src, V_STAGE, &sm.v_full[sv]);
             if (k >= (uint32_t)ar.gst) wait_wd<2000>(&sm.g_empty[sg], gpar ^ 1u, 2, k);
-            if (k >= (uint32_t)ar.gst) FFP_TRACE(0, k - (uint32_t)ar.gst);   // MMAs of stage k - gst have completed (seen by the TMA thread)
             mbar_expect_tx(&sm.g_full[sg], gbytes);
             tma_load_1d(gdst, src + goff, gbytes, &sm.g_full[sg]);
             src += stage_bytes;
@@ -381,58 +337,17 @@ __global__ void __launch_bounds__(Roles<NPW>::THREADS, 1) fp_sweep_i8_kernel(con
           }
         }
       }
-    } else if (wid >= 1) {
-      // Three MMA-issuing warps, one per remaining control warp (= one per SM sub-partition). A single issuing thread
-      // was measured to be the critical path (it never waited: 2900 cycles per stage for 28 MMAs against 1344 of
-      // tensor time): next to producer warps it gets an issue slot only every few cycles. Each issuer owns a set of
-      // accumulators, so no ordering between issuers is needed: every accumulator is written by one thread only, in
-      // program order. The whole warp runs the loop with warp-uniform values (broadcast by shuffle, so that the
-      // compiler keeps descriptors in uniform registers instead of serialising lanes around every MMA) and one
-      // elected lane issues.
-      const bool leader = elect_one();
-      // instruction descriptor: D = s32, A = B = signed 8-bit, both K-major, N = 64, M = 128
-      const uint32_t idesc = (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(NBR >> 3) << 17) | ((128u >> 4) << 24);
-      const uint32_t tmu = __shfl_sync(0xffffffffu, tm, 0);
-      const uint32_t g0 = smem_u32(sm.G), s0 = smem_u32(sm.S);
-      uint32_t k = 0, ps = 0;  // global stage counter; pass counter (one pass = one row group of one item)
-      uint32_t sg = 0, gpar = 0, ss = 0, spar = 0, ga = g0, sa = s0;  // ring positions, parities, slot addresses
-      for (int item = blockIdx.x; item < ar.nwork; item += gridDim.x) {
-        const int pi = ar.pidx[item / ar.ntile];
-        const int rows = __shfl_sync(0xffffffffu, ar.meta[pi].i8_rows, 0);
-        const int nst = __shfl_sync(0xffffffffu, ar.meta[pi].i8_nst, 0);
-        for (int grp = 0; 128 * grp < rows; ++grp, ++ps) {
-          const uint32_t aplane16 = (uint32_t)(min(128, rows - 128 * grp) * KT) >> 4;
-          if (ps > 0) wait_wd<0>(sm.acc_empty, (ps - 1) & 1u, 3, ps);  // the epilogue has drained the accumulators
-          for (int c = 0; c < nst; ++c, ++k) {
-            wait_wd<0>(&sm.g_full[sg], gpar, 4, k);
-            wait_wd<0>(&sm.s_full[ss], spar, 5, k);
-            tc_fence_after();
-            if (wid == 1 && leader) FFP_TRACE(1, k);   // issuer 0 sees stage k complete
-            const uint32_t da_lo = ((ga >> 4) & 0x3fffu) | (1u << 16);
-            const uint32_t db_lo = ((sa >> 4) & 0x3fffu) | (1u << 16);
-            if (leader) {
-              if (wid == 1) issue_stage<0>(tmu, da_lo, db_lo, aplane16, idesc, c == 0);
-              else if (wid == 2) issue_stage<1>(tmu, da_lo, db_lo, aplane16, idesc, c == 0);
-              else issue_stage<2>(tmu, da_lo, db_lo, aplane16, idesc, c == 0);
-              umma_commit(&sm.g_empty[sg]);  // each issuer's commit arrives when ITS MMAs above have read their operands
-              umma_commit(&sm.s_empty[ss]);
-              if (wid == 1) FFP_TRACE(2, k);           // issuer 0 has issued its MMAs of stage k
-            }
-            __syncwarp();
-            if (++sg == (uint32_t)ar.gst) { sg = 0; gpar ^= 1u; ga = g0; } else ga += (uint32_t)ar.gslot;
-            if (++ss == SST) { ss = 0; spar ^= 1u; sa = s0; } else sa += S_STAGE;
-          }
-          if (leader) umma_commit(sm.acc_full);
-          __syncwarp();
-        }
-      }
     }
-  } else if (wid < 8) {
-    // ================= epilogue warpgroup: one TMEM lane quarter per warp =================
-    reg_set_inc<R::REGS_EPI>();
-    const int ew = wid - 4;
-    const int lrow = 32 * ew + lane;   // TMEM lane = operand row inside the row group
-    uint32_t it = 0, ps = 0;  // items; passes (one per row group of an item)
+  } else if (wid < 12) {
+    // ================= consumer warpgroups: wgmma issue + epilogue, 64 operand rows each =================
+    reg_set_inc<REGS_CONS>();
+    const int cwg = (wid - 4) >> 2;          // operand rows 64 cwg .. 64 cwg + 63 of the row group
+    const int cw = (wid - 4) & 3;            // warp inside the warpgroup: 16 of those rows
+    const int lr0 = 64 * cwg + 16 * cw + (lane >> 2);  // accumulator rows lr0 and lr0 + 8 of this thread
+    const uint32_t g0 = smem_u32(sm.G), s0 = smem_u32(sm.S);
+    uint32_t acc[NPL][NACC];
+    uint32_t k = 0, it = 0;
+    uint32_t sg = 0, gpar = 0, ss = 0, spar = 0, ga = g0, sa = s0;  // ring positions, parities, slot addresses
     for (int item = blockIdx.x; item < ar.nwork; item += gridDim.x, ++it) {
       const int gp = item / ar.ntile, ft = item - gp * ar.ntile;
       const int p = ar.pidx[gp];
@@ -440,170 +355,143 @@ __global__ void __launch_bounds__(Roles<NPW>::THREADS, 1) fp_sweep_i8_kernel(con
       const int64_t f0 = (int64_t)ft * NF;
       // bases wider than 127 columns take one pass per group of 128 operand rows; the b-sums of the groups add up in
       // `part`, the w row sits in the last group
-      for (int grp = 0; 128 * grp < pm.i8_rows; ++grp, ++ps) {
-      const int row = 128 * grp + lrow;
-      const double rs = ar.rowscale[(size_t)p * RS + row];
-      const bool has_rows = 128 * grp + 32 * ew < pm.i8_rows;  // warp-uniform
-      wait_wd<100000>(sm.acc_full, ps & 1u, 6, ps);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c0 = 0; c0 < NF; c0 += 8) {
-        double v[24];
-        if (has_rows) {
-          const uint32_t ta = tm + ((uint32_t)(32 * ew) << 16) + (uint32_t)c0;
-          double ysv[8], ycv[8];
-          {
-            uint32_t acc[NPL][8];
-#pragma unroll
-            for (int g = 0; g < NPL; ++g) tmem_ld8(ta + (uint32_t)(g * NBR), acc[g]);
-            tmem_ld_wait();
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              double y = (double)(int)acc[NPL - 1][q];  // smallest weight first
-#pragma unroll
-              for (int g = NPL - 2; g >= 0; --g) y = fma(y, 0.00390625, (double)(int)acc[g][q]);
-              ysv[q] = y * rs;
-            }
+      for (int grp = 0; 128 * grp < pm.i8_rows; ++grp) {
+        const int rows_g = min(128, pm.i8_rows - 128 * grp);
+        const bool active = 64 * cwg < rows_g;  // warpgroup-uniform: this warpgroup's rows exist in the group
+        const uint32_t aplane16 = (uint32_t)(rows_g * KT) >> 4;
+        uint32_t psg = 0, pss = 0;  // slots of the previous stage, released once its MMAs have completed
+        for (int c = 0; c < pm.i8_nst; ++c, ++k) {
+          wait_wd<0>(&sm.g_full[sg], gpar, 4, k);
+          wait_wd<0>(&sm.s_full[ss], spar, 5, k);
+          __syncwarp();  // lanes leave the polling loops independently; the .aligned wgmma instructions need them converged
+          if (active) {
+            wgmma_fence();
+            issue_stage(acc, desc_lo(ga + (uint32_t)(64 * cwg * KT)), desc_lo(sa), aplane16, c == 0);
+            wgmma_commit();
+            wgmma_wait<1>();  // the stage before this one has been read
           }
-          {
-            uint32_t acc[NPL][8];
-#pragma unroll
-            for (int g = 0; g < NPL; ++g) tmem_ld8(ta + (uint32_t)(g * NBR + NF), acc[g]);
-            tmem_ld_wait();
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              double y = (double)(int)acc[NPL - 1][q];
-#pragma unroll
-              for (int g = NPL - 2; g >= 0; --g) y = fma(y, 0.00390625, (double)(int)acc[g][q]);
-              ycv[q] = y * rs;
-            }
-          }
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const double ys = ysv[q], yc = ycv[q];
-            if (row == pm.m) {  // the w row: (s|r) = s.w, (c|r) = c.w  (DESIGN.md section 2)
-              sm.nval[2 * (c0 + q)] = ys;
-              sm.nval[2 * (c0 + q) + 1] = yc;
-            }
-            const bool basis = row < pm.mfix;  // rows of the draw-independent block enter the b-sums (plain Fp: all)
-            if (NMFP && row >= pm.mfix && row < pm.m && f0 + c0 + q < ar.F) {
-              // rows of the per-draw block leave as z' in the layout nmfp_stageB_kernel streams: k-block (row / 4),
-              // column block (4 frequencies), then 16 * {sin, cos} + 4 * (frequency % 4) + row % 4
-              const int jr = row - pm.mfix + (ar.mvpad - pm.mvar), fi = c0 + q;
-              double* z = ar.Z + ((size_t)p * ar.ntile + ft) * ((size_t)ar.mvpad * 64) +
-                          (size_t)(((jr >> 2) * 8 + (fi >> 2)) * 32 + 4 * (fi & 3) + (jr & 3));
-              z[0] = ys;
-              z[16] = yc;
-            }
-            v[3 * q] = basis ? ys * ys : 0.0;
-            v[3 * q + 1] = basis ? ys * yc : 0.0;
-            v[3 * q + 2] = basis ? yc * yc : 0.0;
-          }
-          // transpose-reduce over the 32 rows of this warp: 24 -> 12 -> 6 -> 3 values per lane, then lanes 4q hold
-          // the three sums of frequency c0 + q
-#pragma unroll
-          for (int i = 0; i < 12; ++i) {
-            const bool up = lane & 16;
-            const double keep = up ? v[i + 12] : v[i], send = up ? v[i] : v[i + 12];
-            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-          }
-#pragma unroll
-          for (int i = 0; i < 6; ++i) {
-            const bool up = lane & 8;
-            const double keep = up ? v[i + 6] : v[i], send = up ? v[i] : v[i + 6];
-            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-          }
-#pragma unroll
-          for (int i = 0; i < 3; ++i) {
-            const bool up = lane & 4;
-            const double keep = up ? v[i + 3] : v[i], send = up ? v[i] : v[i + 3];
-            double t = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-            t += __shfl_xor_sync(0xffffffffu, t, 2);
-            t += __shfl_xor_sync(0xffffffffu, t, 1);
-            v[i] = t;
-          }
-        } else {
-          v[0] = v[1] = v[2] = 0.0;
+          if (c > 0 && (tid & 127) == 0) { mbar_arrive(&sm.g_empty[psg]); mbar_arrive(&sm.s_empty[pss]); }
+          psg = sg; pss = ss;
+          if (++sg == (uint32_t)ar.gst) { sg = 0; gpar ^= 1u; ga = g0; } else ga += (uint32_t)ar.gslot;
+          if (++ss == SST) { ss = 0; spar ^= 1u; sa = s0; } else sa += S_STAGE;
         }
-        if ((lane & 3) == 0) {
-          const int q = ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1);
-          double* o = sm.part + ((size_t)ew * NF + c0 + q) * 3;
-          if (grp == 0) { o[0] = v[0]; o[1] = v[1]; o[2] = v[2]; }
-          else { o[0] += v[0]; o[1] += v[1]; o[2] += v[2]; }   // (this warp's own slots: no other writer)
+        if (active) wgmma_wait<0>();
+        if ((tid & 127) == 0) { mbar_arrive(&sm.g_empty[psg]); mbar_arrive(&sm.s_empty[pss]); }
+
+        // ---- epilogue of the pass: thread holds rows lr0, lr0 + 8 x frequencies 8 jn + 2 (lane & 3) + e
+        double v[4][3];  // per frequency slot q = 2 jn + e: the two rows' contributions to the three b-sums
+#pragma unroll
+        for (int q = 0; q < 4; ++q) v[q][0] = v[q][1] = v[q][2] = 0.0;
+        if (active) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int row = 128 * grp + lr0 + 8 * h;
+            const double rs = ar.rowscale[(size_t)p * RS + row];
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+              const int jn = q >> 1, e = q & 1;
+              const int is = 4 * jn + 2 * h + e, ic = is + 8;  // sin column 8 jn + .., cos column 16 + the same
+              double ys = (double)(int)acc[NPL - 1][is], yc = (double)(int)acc[NPL - 1][ic];  // smallest weight first
+#pragma unroll
+              for (int g = NPL - 2; g >= 0; --g) {
+                ys = fma(ys, 0.00390625, (double)(int)acc[g][is]);
+                yc = fma(yc, 0.00390625, (double)(int)acc[g][ic]);
+              }
+              ys *= rs;
+              yc *= rs;
+              const int fl = 8 * jn + 2 * (lane & 3) + e;  // frequency inside the tile
+              if (row == pm.m) {  // the w row: (s|r) = s.w, (c|r) = c.w  (DESIGN.md section 2)
+                sm.nval[2 * fl] = ys;
+                sm.nval[2 * fl + 1] = yc;
+              }
+              if (NMFP && row >= pm.mfix && row < pm.m && f0 + fl < ar.F) {
+                // rows of the per-draw block leave as z' in the layout nmfp_stageB_kernel streams: 32-frequency tile,
+                // k-block (row / 4), column block (4 frequencies), then 16 * {sin, cos} + 4 * (frequency % 4) + row % 4
+                const int jr = row - pm.mfix + (ar.mvpad - pm.mvar), fi = (int)((f0 + fl) & 31);
+                double* z = ar.Z + ((size_t)p * ar.nt32 + (size_t)((f0 + fl) >> 5)) * ((size_t)ar.mvpad * 64) +
+                            (size_t)(((jr >> 2) * 8 + (fi >> 2)) * 32 + 4 * (fi & 3) + (jr & 3));
+                z[0] = ys;
+                z[16] = yc;
+              }
+              if (row < pm.mfix) {  // rows of the draw-independent block enter the b-sums (plain Fp: all)
+                v[q][0] = fma(ys, ys, v[q][0]);
+                v[q][1] = fma(ys, yc, v[q][1]);
+                v[q][2] = fma(yc, yc, v[q][2]);
+              }
+            }
+          }
+        }
+        // sum over the 8 lanes that share (lane & 3): the 16 rows of this warp
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+#pragma unroll
+          for (int k2 = 0; k2 < 3; ++k2) {
+            double t = v[q][k2];
+            t += __shfl_xor_sync(0xffffffffu, t, 4);
+            t += __shfl_xor_sync(0xffffffffu, t, 8);
+            t += __shfl_xor_sync(0xffffffffu, t, 16);
+            v[q][k2] = t;
+          }
+        if (lane < 4) {
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const int fl = 8 * (q >> 1) + 2 * lane + (q & 1);
+            double* o = sm.part + ((size_t)(wid - 4) * NF + fl) * 3;
+            if (grp == 0) { o[0] = v[q][0]; o[1] = v[q][1]; o[2] = v[q][2]; }
+            else { o[0] += v[q][0]; o[1] += v[q][1]; o[2] += v[q][2]; }   // (this warp's own slots: no other writer)
+          }
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(sm.acc_empty);  // tensor memory may be overwritten by the next pass
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");  // partial sums and the w-row values of the 4 warps are visible
+      asm volatile("bar.sync 1, 256;" ::: "memory");  // partial sums and the w-row values of the 8 warps are visible
       const uint32_t buf = it & 1u;
-      if (ew == 0) {
+      if (wid == 4) {
         wait_wd<2000>(&sm.sums_full[buf], (it >> 1) & 1u, 7, it);
-        const int f = lane;
-        const int64_t fidx = f0 + f;
-        double b[3] = {0, 0, 0}, a[3];
+        if (lane < NF) {
+          const int f = lane;
+          const int64_t fidx = f0 + f;
+          double b[3] = {0, 0, 0}, a[3];
 #pragma unroll
-        for (int w2 = 0; w2 < 4; ++w2)
+          for (int w2 = 0; w2 < 8; ++w2)
 #pragma unroll
-          for (int k2 = 0; k2 < 3; ++k2) b[k2] += sm.part[((size_t)w2 * NF + f) * 3 + k2];
+            for (int k2 = 0; k2 < 3; ++k2) b[k2] += sm.part[((size_t)w2 * NF + f) * 3 + k2];
 #pragma unroll
-        for (int k2 = 0; k2 < 2; ++k2) {
-          a[k2] = sm.redA[((buf * 2 + 0) * NF + f) * 3 + k2];
-          if (NG == 2) a[k2] += sm.redA[((buf * 2 + 1) * NF + f) * 3 + k2];
-        }
-        a[2] = pm.ninv_sum - a[0];  // c N^-1 c = sum 1/N - s N^-1 s (s^2 + c^2 = 1 to the last bit of the sincos values)
-        const double N0 = sm.nval[2 * f], N1 = sm.nval[2 * f + 1];
-        // M = [[ss, sc],[sc, cc]], N = [n0, n1]; LU with partial pivoting
-        double m00 = a[0] - b[0], m01 = a[1] - b[1], m10 = m01, m11 = a[2] - b[2];
-        double n0 = N0, n1 = N1;
-        if (fabs(m10) > fabs(m00)) {  // row swap; the unknowns keep their order
-          double t0 = m00; m00 = m10; m10 = t0;
-          t0 = m01; m01 = m11; m11 = t0;
-          t0 = n0; n0 = n1; n1 = t0;
-        }
-        const double lq = m10 / m00;
-        const double u = m11 - lq * m01;
-        const double x1 = (n1 - lq * n0) / u;
-        const double x0 = (n0 - m01 * x1) / m00;
-        double val = 0.5 * (N0 * x0 + N1 * x1);
-        if (NMFP) {
-          if (fidx < ar.F) {  // the draw-independent pieces (fixed block removed) for stage B
-            double* o = ar.A + ((size_t)p * ar.ntile + ft) * 160 + f;
-            o[0] = a[0] - b[0]; o[32] = a[1] - b[1]; o[64] = a[2] - b[2]; o[96] = N0; o[128] = N1;
-          }
-        } else if (fidx < ar.F) {
-          if (!(ar.freqs[fidx] > 0.0)) val = __longlong_as_double(0x7ff8000000000000LL);  // f <= 0: NaN like f**(1/3)
-          if (ar.terms) ar.terms[(size_t)p * ar.F + fidx] = val;
-          if (ar.inner) {
-            double* o = ar.inner + ((size_t)p * ar.F + fidx) * 5;
-            o[0] = a[0] - b[0]; o[1] = a[1] - b[1]; o[2] = a[2] - b[2]; o[3] = N0; o[4] = N1;
+          for (int k2 = 0; k2 < 2; ++k2)
+            a[k2] = sm.redA[((buf * 2 + 0) * NF + f) * 3 + k2] + sm.redA[((buf * 2 + 1) * NF + f) * 3 + k2];
+          a[2] = pm.ninv_sum - a[0];  // c N^-1 c = sum 1/N - s N^-1 s (s^2 + c^2 = 1 to the last bit of the sincos values)
+          const double N0 = sm.nval[2 * f], N1 = sm.nval[2 * f + 1];
+          // M = [[ss, sc],[sc, cc]], N = [(s|r), (c|r)]
+          double val = term_2x2(a[0] - b[0], a[1] - b[1], a[2] - b[2], N0, N1);
+          if (NMFP) {
+            if (fidx < ar.F) {  // the draw-independent pieces (fixed block removed) for stage B
+              double* o = ar.A + ((size_t)p * ar.nt32 + (size_t)(fidx >> 5)) * 160 + (fidx & 31);
+              o[0] = a[0] - b[0]; o[32] = a[1] - b[1]; o[64] = a[2] - b[2]; o[96] = N0; o[128] = N1;
+            }
+          } else if (fidx < ar.F) {
+            if (!(ar.freqs[fidx] > 0.0)) val = __longlong_as_double(0x7ff8000000000000LL);  // f <= 0: NaN like f**(1/3)
+            if (ar.terms) ar.terms[(size_t)p * ar.F + fidx] = val;
+            if (ar.inner) {
+              double* o = ar.inner + ((size_t)p * ar.F + fidx) * 5;
+              o[0] = a[0] - b[0]; o[1] = a[1] - b[1]; o[2] = a[2] - b[2]; o[3] = N0; o[4] = N1;
+            }
           }
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(&sm.sums_empty[buf]);
       }
-      asm volatile("bar.sync 1, 128;" ::: "memory");  // part / nval are rewritten by the next item
+      asm volatile("bar.sync 1, 256;" ::: "memory");  // part / nval are rewritten by the next item
     }
   } else {
-    // ================= producers: sin/cos digit planes + the three quadratic sums =================
-    if (NPW == 16) reg_set_dec<R::REGS_PROD>();
-    else reg_set_inc<R::REGS_PROD>();
-    const int pw = wid - 8;
-    const uint32_t grp = (uint32_t)(pw >> 3);          // serves the stages with (global stage index % NG) == grp
+    // ================= producers: sin/cos digit planes + the two quadratic sums =================
+    reg_set_dec<REGS_PROD>();
+    const int pw = wid - 12;
+    const uint32_t grp = (uint32_t)(pw >> 2);          // serves the stages with (global stage index % 2) == grp
     // lane = 4 * kg + fl: the 8 lanes of a quarter-warp read two distinct (t, 1/N) entries 64 bytes apart (no bank
     // conflict on the 16-byte loads), and a warp's 4-byte stores cover 4 rows x 32 bytes = all 32 banks
     const int kg = lane >> 2, fl = lane & 3;
-    const int f = 4 * (pw & 7) + fl;                   // frequency inside the tile
-    const int soff = swz32(f, 4 * kg);                 // word of TOAs 4kg..4kg+3 in row f (sin); cos row: + 1024
-    // The schedule is built around one hardware fact: fp64 arithmetic and tcgen05 MMAs share a resource on the SM
-    // (tools/probes/umma_fp64_overlap_probe.cu: back-to-back MMAs starve DFMAs; tools/i8_trace.py: next to each other
-    // the fp64 part of a stage runs at a quarter of the fp64 rate and the MMAs at ~70 %), and a warp stalled on the fp64
-    // pipe cannot issue its integer work either. Conversions, integer work and stores are free underneath the MMAs. So
-    // a group announces stage k (s_full) not when its planes are stored but after the fp64 part of its NEXT stage: the
-    // MMAs of stage k then start next to the integer part of stage k + NG (digits, byte transpose, stores) instead of
-    // next to an fp64 part. Measured alternatives (announce at once, integer part interleaved into the next fp64 part,
-    // strictly exclusive phases, batches and coarse phases of several stages): DESIGN.md section 4b.
+    const int f = 4 * (pw & 3) + fl;                   // frequency inside the tile
+    const int soff = swz32(f, 4 * kg);                 // word of TOAs 4kg..4kg+3 in row f (sin); cos row: + NF rows
+    // A group announces stage k (s_full) after the fp64 part of its NEXT stage, so that the MMAs of stage k run next to
+    // the integer part of stage k + 2 (digits, byte transpose, stores) rather than next to an fp64 part.
     auto store_planes = [&](const double (&sv4)[4], const double (&cv4)[4], unsigned char* sb) {
       uint32_t slo[4], shi[4], clo[4], chi[4];
 #pragma unroll
@@ -626,7 +514,7 @@ __global__ void __launch_bounds__(Roles<NPW>::THREADS, 1) fp_sweep_i8_kernel(con
         *reinterpret_cast<uint32_t*>(sb + 0 * S_PLANE) = __byte_perm(f2, h2, 0x5410);  // byte 6
       }
       {
-        unsigned char* cb = sb + NF * KT;  // cos rows 32..63
+        unsigned char* cb = sb + NF * KT;  // cos rows NF..2NF-1
         const uint32_t a = __byte_perm(clo[0], clo[1], 0x5140), b = __byte_perm(clo[0], clo[1], 0x7362);
         const uint32_t c2 = __byte_perm(clo[2], clo[3], 0x5140), d = __byte_perm(clo[2], clo[3], 0x7362);
         const uint32_t e2 = __byte_perm(chi[0], chi[1], 0x5140), f2 = __byte_perm(chi[0], chi[1], 0x7362);
@@ -654,13 +542,12 @@ __global__ void __launch_bounds__(Roles<NPW>::THREADS, 1) fp_sweep_i8_kernel(con
       // one pass over the TOAs per group of 128 operand rows (bases wider than 127 columns): the planes are produced
       // again for every pass, the quadratic sums only in the first
       for (int rg = 0; 128 * rg < pm.i8_rows; ++rg, kbase += (uint32_t)nst) {
-      const int c0 = NG == 1 ? 0 : (int)((kbase ^ grp) & 1u);
-      for (int c = c0; c < nst; c += NG) {
+      const int c0 = (int)((kbase ^ grp) & 1u);
+      for (int c = c0; c < nst; c += 2) {
         const uint32_t k = kbase + (uint32_t)c;
         const uint32_t sv = k % VST, ss = k % SST;
         wait_wd<2000>(&sm.v_full[sv], (k / VST) & 1u, 8, k);
         const double2* vv = reinterpret_cast<const double2*>(sm.V + sv * V_STAGE) + 4 * kg;
-        if (pw == 0 && lane == 0) FFP_TRACE(3, k);   // fp64 part of stage k starts (inputs present)
         // ---- fp64 part: four (TOA, frequency) pairs per thread
         double ph[4], ninv[4], sv4[4], cv4[4];
 #pragma unroll
@@ -691,7 +578,6 @@ __global__ void __launch_bounds__(Roles<NPW>::THREADS, 1) fp_sweep_i8_kernel(con
         // ---- the group's previous stage is complete in shared memory: announce it now (see above)
         __syncwarp();
         if (lane == 0) {
-          if (pw == 0) FFP_TRACE(4, k);              // fp64 part of stage k done
           mbar_arrive(&sm.v_empty[sv]);
           if (pend >= 0) mbar_arrive(&sm.s_full[pend]);
         }
@@ -699,7 +585,6 @@ __global__ void __launch_bounds__(Roles<NPW>::THREADS, 1) fp_sweep_i8_kernel(con
         if (k >= SST) wait_wd<2000>(&sm.s_empty[ss], ((k / SST) - 1) & 1u, 9, k);
         store_planes(sv4, cv4, sm.S + ss * S_STAGE + soff);
         fence_proxy_async();  // generic-proxy stores -> visible to the tensor core's (async proxy) operand reads
-        if (pw == 0 && lane == 0) FFP_TRACE(5, k);   // planes of stage k stored
         pend = (int)ss;
       }
       }
@@ -724,51 +609,76 @@ __global__ void __launch_bounds__(Roles<NPW>::THREADS, 1) fp_sweep_i8_kernel(con
     __syncwarp();
     if (lane == 0 && pend >= 0) mbar_arrive(&sm.s_full[pend]);  // the group's last stage of this CTA
   }
-  tc_fence_before();
   __syncthreads();
-  if (wid == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tm), "n"(512));
 }
 
 // ---- measurement helper: the tensor path's own ceilings (fastfp_fp64_peak kinds 17 and 18) -----------------------
-// Back-to-back kind::i8 MMAs from one thread per CTA, one CTA per SM, operands in the sweep kernel's SWIZZLE_32B planes:
-// N = 256 gives the INT8 tensor peak of the chip, N = 64 with the sweep's 28-product stage gives the rate this
-// formulation can reach at most (an M=128, N=64 MMA is bound by its 6 KB of shared-memory operand reads).
+// Back-to-back s8 wgmmas from two warpgroups per CTA (128 operand rows), one CTA per SM, operands in the sweep
+// kernel's SWIZZLE_32B planes: N = 256 (one accumulator) gives the INT8 tensor peak of the chip, N = 32 with the
+// sweep's 28-product stage into 7 accumulators gives the rate this formulation can reach at most.
+__device__ __forceinline__ void wgmma_i8_n256(uint32_t (&d)[128], uint64_t da, uint64_t db) {
+#define R8(i) "+r"(d[i]), "+r"(d[i + 1]), "+r"(d[i + 2]), "+r"(d[i + 3]), "+r"(d[i + 4]), "+r"(d[i + 5]), "+r"(d[i + 6]), "+r"(d[i + 7])
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n256k32.s32.s8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, 1;\n"
+      : R8(0), R8(8), R8(16), R8(24), R8(32), R8(40), R8(48), R8(56), R8(64), R8(72), R8(80), R8(88), R8(96), R8(104),
+        R8(112), R8(120)
+      : "l"(da), "l"(db));
+#undef R8
+}
+
 template <int N>
-__global__ void __launch_bounds__(64, 1) i8_peak_kernel(int iters, int* out) {
+__global__ void __launch_bounds__(256, 1) i8_peak_kernel(int iters, int* out) {
   extern __shared__ __align__(1024) unsigned char smem[];
-  __shared__ uint32_t tmem_base;
-  __shared__ __align__(8) uint64_t bar;
   constexpr int A_PLANE = 128 * KT, B_PLANE = N * KT;
   unsigned char* sA = smem;
   unsigned char* sB = smem + NPL * A_PLANE;
   for (int i = threadIdx.x; i < NPL * (A_PLANE + B_PLANE); i += blockDim.x) smem[i] = (unsigned char)((i * 7 + 3) & 3);
-  if (threadIdx.x < 32) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(&tmem_base)), "n"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n");
-  }
-  if (threadIdx.x == 0) { mbar_init(&bar, 1); fence_barrier_init(); }
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tm = tmem_base;
-  if (threadIdx.x == 0) {
-    const uint32_t idesc = (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((128u >> 4) << 24);
+  const uint32_t a_lo = desc_lo(smem_u32(sA) + (uint32_t)((threadIdx.x >> 7) * 64 * KT)), b_lo = desc_lo(smem_u32(sB));
+  uint32_t sum = 0;
+  if (N == 256) {
+    uint32_t d[128];
+#pragma unroll
+    for (int i = 0; i < 128; ++i) d[i] = 0;
+    wgmma_fence();
     for (int it = 0; it < iters; ++it) {
 #pragma unroll
       for (int i = 0; i < NPL; ++i)
 #pragma unroll
         for (int j = 0; j < NPL - i; ++j)
-          umma_i8(tm + (uint32_t)(((i + j) * N) % 512), umma_desc(smem_u32(sA + i * A_PLANE)),
-                  umma_desc(smem_u32(sB + j * B_PLANE)), idesc, (it > 0 || i > 0) ? 1u : 0u);
+          wgmma_i8_n256(d, DESC_HI | (uint64_t)(a_lo + (uint32_t)(i * A_PLANE / 16)),
+                        DESC_HI | (uint64_t)(b_lo + (uint32_t)(j * B_PLANE / 16)));
+      wgmma_commit();
+      wgmma_wait<1>();
     }
-    umma_commit(&bar);
-    wait_wd<0>(&bar, 0u, 11, 0u);
-    if (out) out[blockIdx.x] = 1;
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < 128; ++i) sum += d[i];
+  } else {
+    uint32_t acc[NPL][NACC];
+    wgmma_fence();
+    for (int it = 0; it < iters; ++it) {
+      issue_stage(acc, a_lo, b_lo, A_PLANE / 16, it == 0);
+      wgmma_commit();
+      wgmma_wait<1>();
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int g = 0; g < NPL; ++g)
+#pragma unroll
+      for (int i = 0; i < NACC; ++i) sum += acc[g][i];
   }
-  tc_fence_before();
-  __syncthreads();
-  if (threadIdx.x < 32) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tm), "n"(512));
+  if (out) out[blockIdx.x * blockDim.x + threadIdx.x] = (int)sum;
 }
 
 }  // namespace i8
@@ -778,18 +688,18 @@ int run_i8_peak(int kind, int iters, double* tops, double* ms_out) {
   int dev = 0, sms = 0;
   FFP_CUDA(cudaGetDevice(&dev));
   FFP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const int N = kind == 17 ? 256 : 64;
+  const int N = kind == 17 ? 256 : 32;
   const size_t smem = (size_t)NPL * (128 + N) * KT + 1024;
   if (kind == 17) FFP_CUDA(cudaFuncSetAttribute(i8_peak_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  else FFP_CUDA(cudaFuncSetAttribute(i8_peak_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  else FFP_CUDA(cudaFuncSetAttribute(i8_peak_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   cudaEvent_t e0, e1;
   FFP_CUDA(cudaEventCreate(&e0));
   FFP_CUDA(cudaEventCreate(&e1));
   float best = 1e30f;
   for (int rep = 0; rep < 4; ++rep) {
     FFP_CUDA(cudaEventRecord(e0));
-    if (kind == 17) i8_peak_kernel<256><<<sms, 64, smem>>>(iters, nullptr);
-    else i8_peak_kernel<64><<<sms, 64, smem>>>(iters, nullptr);
+    if (kind == 17) i8_peak_kernel<256><<<sms, 256, smem>>>(iters, nullptr);
+    else i8_peak_kernel<32><<<sms, 256, smem>>>(iters, nullptr);
     FFP_CUDA(cudaEventRecord(e1));
     FFP_CUDA(cudaEventSynchronize(e1));
     float ms = 0;
@@ -918,59 +828,26 @@ int launch_fp_sweep_i8(const fastfp_pack* pk, const double* d_freqs, int64_t F, 
   if (nwork > 0x7fffffffLL) { set_error("frequency batch too large for one launch"); return -1; }
   a.ntile = (int)ntile;
   a.nwork = (int)nwork;
+  a.nt32 = (int)((F + 31) / 32);
   a.gslot = NPL * (pk->i8_rows_max < 128 ? pk->i8_rows_max : 128) * KT;  // one row group
   const size_t budget = 220 * 1024 - SMEM_FIXED;
   int gst = (int)(budget / a.gslot);
   gst = gst > 8 ? 8 : gst;
-  // the last plane of the last slot is read 128 rows deep: the S ring behind the G ring absorbs the overrun
+  // the last plane of the last slot is read 64 rows deep per warpgroup: the S ring behind the G ring absorbs the overrun
   if (gst < 2) { set_error("internal: no room for the G ring"); return FASTFP_ERR_UNSUPPORTED; }
   a.gst = gst;
   const size_t smem = (size_t)gst * a.gslot + SMEM_FIXED;
   static bool attr_done[64] = {};
   if (!attr_done[pk->device & 63]) {
-#define FFP_I8_ATTR(NPW_)                                                                                             \
-  FFP_CUDA(cudaFuncSetAttribute(fp_sweep_i8_kernel<false, NPW_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)); \
-  FFP_CUDA(cudaFuncSetAttribute(fp_sweep_i8_kernel<true, NPW_>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    FFP_I8_ATTR(16) FFP_I8_ATTR(8)
-#undef FFP_I8_ATTR
+    FFP_CUDA(cudaFuncSetAttribute(fp_sweep_i8_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    FFP_CUDA(cudaFuncSetAttribute(fp_sweep_i8_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_done[pk->device & 63] = true;
   }
   const unsigned grid = (unsigned)(nwork < pk->num_sms ? nwork : pk->num_sms);
-  // producer warps per CTA: 16 (two groups alternating stages; default, C2 18.0 ms) or 8 (FASTFP_B200_I8_NPW=8: 19.2 ms)
-#ifdef FFP_I8_TRACE
-  long long* d_trace = nullptr;
-  const char* trace_path = getenv("FASTFP_B200_I8_TRACE");
-  if (trace_path) {
-    FFP_CUDA(cudaMalloc(&d_trace, sizeof(long long) * TRACE_EV * TRACE_K));
-    FFP_CUDA(cudaMemsetAsync(d_trace, 0, sizeof(long long) * TRACE_EV * TRACE_K, st));
-  }
-  a.trace = d_trace;
-#endif
-  static const int npw = getenv("FASTFP_B200_I8_NPW") ? atoi(getenv("FASTFP_B200_I8_NPW")) : 16;
-  if (npw == 16) {
-    if (nm) fp_sweep_i8_kernel<true, 16><<<grid, Roles<16>::THREADS, smem, st>>>(a);
-    else fp_sweep_i8_kernel<false, 16><<<grid, Roles<16>::THREADS, smem, st>>>(a);
-  } else {
-    if (nm) fp_sweep_i8_kernel<true, 8><<<grid, Roles<8>::THREADS, smem, st>>>(a);
-    else fp_sweep_i8_kernel<false, 8><<<grid, Roles<8>::THREADS, smem, st>>>(a);
-  }
+  if (nm) fp_sweep_i8_kernel<true><<<grid, THREADS, smem, st>>>(a);
+  else fp_sweep_i8_kernel<false><<<grid, THREADS, smem, st>>>(a);
   g_launches += 1;
   FFP_CUDA(cudaGetLastError());
-#ifdef FFP_I8_TRACE
-  if (d_trace) {  // diagnostic build only: synchronous dump of CTA 0's event clocks
-    std::vector<long long> h((size_t)TRACE_EV * TRACE_K);
-    FFP_CUDA(cudaStreamSynchronize(st));
-    FFP_CUDA(cudaMemcpy(h.data(), d_trace, h.size() * sizeof(long long), cudaMemcpyDeviceToHost));
-    FFP_CUDA(cudaFree(d_trace));
-    if (FILE* fh = fopen(trace_path, "w")) {
-      for (int k = 0; k < TRACE_K; ++k) {
-        for (int e = 0; e < TRACE_EV; ++e) fprintf(fh, "%lld ", h[(size_t)e * TRACE_K + k]);
-        fprintf(fh, "\n");
-      }
-      fclose(fh);
-    }
-  }
-#endif
   return 0;
 }
 

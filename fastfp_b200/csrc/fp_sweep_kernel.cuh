@@ -499,19 +499,8 @@ __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>&
         o[96] = a[3];
         o[128] = a[4];
       } else {
-        // M = [[ss, sc],[sc, cc]], N = [n0, n1]; LU with partial pivoting
-        double m00 = a[0] - b[0], m01 = a[1] - b[1], m10 = m01, m11 = a[2] - b[2];
-        double n0 = a[3], n1 = a[4];
-        if (fabs(m10) > fabs(m00)) {  // row swap; the unknowns keep their order
-          double t0 = m00; m00 = m10; m10 = t0;
-          t0 = m01; m01 = m11; m11 = t0;
-          t0 = n0; n0 = n1; n1 = t0;
-        }
-        const double lq = m10 / m00;
-        const double u = m11 - lq * m01;
-        const double x1 = (n1 - lq * n0) / u;
-        const double x0 = (n0 - m01 * x1) / m00;
-        double val = 0.5 * (a[3] * x0 + a[4] * x1);
+        // M = [[ss, sc],[sc, cc]], N = [(s|r), (c|r)]
+        double val = term_2x2(a[0] - b[0], a[1] - b[1], a[2] - b[2], a[3], a[4]);
         if (!(sm.fq[tid] > 0.0)) val = __longlong_as_double(0x7ff8000000000000LL);
         if (ar.terms) ar.terms[(size_t)p * ar.F + fidx] = val;
         if (ar.inner) {  // the inner products themselves (no f^(-1/3) prefactor: it cancels in every statistic)

@@ -265,7 +265,7 @@ __global__ void __launch_bounds__(768, 1) warp_mix_kernel(int iters, double seed
 
 // kind 16: legacy INT8 tensor MMA (mma.sync.m16n8k32.s8, int32 accumulation) from registers -- how far the
 // warp-level MMA path gets on its own; the split-precision plan of DESIGN.md section 8 needs ~36 such products
-// per fp64 product, so it pays only if this rate (or tcgen05's) is well above 36x the fp64 pipe.
+// per fp64 product, so it pays only if this rate (or wgmma's) is well above 36x the fp64 pipe.
 __global__ void __launch_bounds__(256) imma_peak_kernel(int iters, int seed, double* sink) {
   int c[8][4];
 #pragma unroll

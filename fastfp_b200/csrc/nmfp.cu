@@ -549,21 +549,11 @@ __global__ void __launch_bounds__(StageBCfg<NMBV>::THREADS, 1) nmfp_stageB_kerne
     if ((lane >> 2) == dl) { k0 = r5[0]; k1 = r5[1]; k2 = r5[2]; k3 = r5[3]; k4 = r5[4]; }
     if (dl == nd - 1) {  // uniform: the draws of pulsar p are complete
       const double* a = Ab + (buf * NH + h) * 160 + fi;
-      double m00 = a[0] - k0, m01 = a[32] - k1, m10 = m01, m11 = a[64] - k2;
+      const double m00 = a[0] - k0, m01 = a[32] - k1, m11 = a[64] - k2;
       const double N0 = a[96] - k3, N1 = a[128] - k4;
       __syncwarp();
       if (lane == 0) mbar_arrive(&zempty[buf]);  // z' tile and a-terms of pulsar p are consumed
-      double n0 = N0, n1 = N1;
-      if (fabs(m10) > fabs(m00)) {  // LU with partial pivoting (jnp.linalg.solve, nmfp.py:117)
-        double t0 = m00; m00 = m10; m10 = t0;
-        t0 = m01; m01 = m11; m11 = t0;
-        t0 = n0; n0 = n1; n1 = t0;
-      }
-      const double lq = m10 / m00;
-      const double u = m11 - lq * m01;
-      const double x1 = (n1 - lq * n0) / u;
-      const double x0 = (n0 - m01 * x1) / m00;
-      fpacc += 0.5 * (N0 * x0 + N1 * x1);  // pulsar sum in pulsar order, starting from 0 (nmfp.py:98,117)
+      fpacc += term_2x2(m00, m01, m11, N0, N1);  // pulsar sum in pulsar order, starting from 0 (nmfp.py:98,117)
     }
   }
   if ((lane >> 2) < nd && f < ar.F) {

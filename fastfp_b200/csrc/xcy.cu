@@ -8,12 +8,13 @@
 
 namespace ffp {
 
-// work layout (doubles): LU[m*m] | TNx[m] | TNy[m] | sol[m] | xNy[1]
+// work layout (doubles): LU[m*m] | TNx[m] | TNy[m] | sol[m] | xNy[1]. The threads exchange values through `work`
+// across __syncthreads(), so it must not be __restrict__: that would let the compiler move its loads across the
+// barriers.
 __global__ void xcy_kernel(int64_t n, int m, const double* __restrict__ Nvec,
                            const double* __restrict__ T, const double* __restrict__ sigma,
                            const double* __restrict__ x, const double* __restrict__ y,
-                           const double* __restrict__ x0, double* __restrict__ work,
-                           double* __restrict__ out) {
+                           const double* __restrict__ x0, double* work, double* out) {
   double* LU = work;
   double* TNx = work + (size_t)m * m;
   double* TNy = TNx + m;

@@ -1,7 +1,7 @@
 """``FastFp`` -- drop-in for the reference's ``fastfp.fastfp.FastFp`` (``fastfp/fastfp.py:22-101``).
 
 Same constructor and call signatures; the JAX/XLA program behind ``calculate_Fp`` is replaced
-by the sm_100a sweep kernel of ``libfastfp_b200.so`` reached through the C ABI. Differences a
+by the sm_90a sweep kernel of ``libfastfp_b200.so`` reached through the C ABI. Differences a
 caller can see, all additive:
 
 * ``fgw`` may be a scalar (reference semantics, returns a float) **or** a 1-D array of
@@ -127,8 +127,9 @@ class FastFp(_PackCache):
     :param pta: stored and never used in compute, as in the reference (``fastfp.py:42``)
     :param device: CUDA device ordinal (extension; default 0 or ``LOCAL_RANK``)
     :param path: which kernel sweeps (extension): ``"auto"`` (default; also from ``FASTFP_B200_PATH``) = the
-        INT8 tensor-core kernel (``tcgen05``, exact digit-plane product) when every pulsar fits its tile,
-        else the fp64 DMMA kernel; ``"fp64"`` / ``"i8"`` force one (``"i8"`` raises if the pack cannot take it).
+        fp64 DMMA kernel, the faster one on an H100; ``"prefer-i8"`` = the INT8 tensor-core kernel (``wgmma``,
+        exact digit-plane product) for every pulsar that fits its tile, the fp64 kernel for the rest;
+        ``"fp64"`` / ``"i8"`` force one (``"i8"`` raises if the pack cannot take it).
         Both meet the same parity bar; see DESIGN.md.
     """
 
@@ -158,10 +159,12 @@ class FastFp(_PackCache):
         else:
             pack = _cabi.Pack.create_fp(self.toas, self.residuals, Nvecs, Ts, sigmas, device=self.device)
         if self.path == "prefer-i8":  # the tensor kernel where the pack can take it, silently the fp64 one otherwise
-            try:
-                pack.set_path("i8")
-            except _cabi.FastFpError:
-                pass
+            for p in ("i8", "mixed"):
+                try:
+                    pack.set_path(p)
+                    break
+                except _cabi.FastFpError:
+                    pass
         elif self.path != "auto":
             pack.set_path(self.path)
         return pack

@@ -1,4 +1,4 @@
-"""``FastFe`` -- the Fe-statistic on the B200 engine.
+"""``FastFe`` -- the Fe-statistic on the fastfp_b200 engine.
 
 The reference lists the Fe-statistic as a to-do (``README.md:23``); ``enterprise_extensions.frequentist.FeStat`` is the
 implementation users have today. Fe (Ellis, Siemens & Creighton 2012) is the coherent Earth-term counterpart of Fp: for

@@ -206,7 +206,7 @@ class NMFP(_PackCache):
     :param rn_sigs: one :class:`RN_container` per pulsar
     :param device: CUDA device ordinal (extension; default ``LOCAL_RANK`` or 0)
     :param path: kernel of the draw-independent stage A, like :class:`FastFp`'s ``path`` (``"auto"`` / ``"fp64"`` /
-        ``"i8"``; default from ``FASTFP_B200_PATH``)"""
+        ``"i8"`` / ``"prefer-i8"``; default from ``FASTFP_B200_PATH``)"""
 
     def __init__(self, psrs, rn_sigs, device=None, path=None):
         self.psrs = psrs
@@ -253,10 +253,12 @@ class NMFP(_PackCache):
             pack = _cabi.Pack.create_nmfp(self.toas, self.residuals, Nvecs, Ts, TNTs, m_fix,
                                           [1.0 / f for f in fixed], device=self.device)
         if self.path == "prefer-i8":  # the tensor kernel where the pack can take it, silently the fp64 one otherwise
-            try:
-                pack.set_path("i8")
-            except _cabi.FastFpError:
-                pass
+            for p in ("i8", "mixed"):
+                try:
+                    pack.set_path(p)
+                    break
+                except _cabi.FastFpError:
+                    pass
         elif self.path != "auto":
             pack.set_path(self.path)
         return pack

@@ -76,14 +76,15 @@ int fastfp_fp_sweep(const fastfp_pack_t* pack, const double* freqs, int64_t F, d
 /* Which kernel runs the frequency sweep of this pack (the plain-Fp sweep, the Fe sweep, stage A of nmfp). Both
  * compute the same quantities to the same parity bar:
  *   FASTFP_PATH_I8    the tensor-core kernel: Y = G [s c] as an error-free product of 8-bit digit planes
- *                     (tcgen05.mma kind::i8, exact int32 accumulation in tensor memory), 1.4-3.6x faster;
- *                     takes pulsars with m <= 639 basis columns, n <= 16384 TOAs and finite data in packs with a
- *                     diagonal N (fastfp_pack_set_path(I8) returns FASTFP_ERR_UNSUPPORTED unless EVERY pulsar fits);
+ *                     (wgmma s8 x s8, exact int32 accumulation); takes pulsars with m <= 639 basis columns,
+ *                     n <= 16384 TOAs and finite data in packs with a diagonal N (fastfp_pack_set_path(I8) returns
+ *                     FASTFP_ERR_UNSUPPORTED unless EVERY pulsar fits);
+ *   FASTFP_PATH_MIXED the tensor kernel for the pulsars it takes, the fp64 kernel for the others of the same pack in
+ *                     the same sweep (FASTFP_ERR_UNSUPPORTED if it takes none);
  *   FASTFP_PATH_FP64  the fp64 DMMA kernel (always available; block-N packs use it);
- *   FASTFP_PATH_AUTO  (default) the tensor kernel for the pulsars it takes, the fp64 kernel for the others of the
- *                     same pack in the same sweep.
- * fastfp_pack_path returns the path in effect (never AUTO): FP64, I8 (all pulsars) or MIXED (AUTO with some
- * pulsars on either kernel). */
+ *   FASTFP_PATH_AUTO  (default) the fp64 DMMA kernel, the faster of the two on an H100.
+ * fastfp_pack_path returns the path in effect (never AUTO): FP64, I8 (all pulsars) or MIXED (some pulsars on
+ * either kernel). */
 #define FASTFP_PATH_AUTO 0
 #define FASTFP_PATH_FP64 1
 #define FASTFP_PATH_I8 2
@@ -222,8 +223,8 @@ int fastfp_xcy_blockn(int device, int64_t n, int64_t m, const double* Nvec, cons
  * kind 1 as the measured fp64-pipe denominator (MEASURED_PEAKS.json has no fp64 figure). Kinds 3-12
  * are the kernel-design probes of csrc/microbench.cu; 13-15 run the sweep kernel's warp
  * specialisation (8 DMMA warps + 16 DFMA warps) on registers only; 16 = legacy INT8 mma.sync rate
- * (reported as 2 x MAC/s in the same unit); 17 = tcgen05.mma kind::i8 M=128 N=256 (the INT8 tensor peak, TOP/s);
- * 18 = the tensor sweep's own stage (28 plane products M=128 N=64 K=32: bound by shared-memory operand reads). */
+ * (reported as 2 x MAC/s in the same unit); 17 = s8 wgmma m64n256k32 on two warpgroups (the INT8 tensor peak, TOP/s);
+ * 18 = the tensor sweep's own stage (28 plane products, two warpgroups of m64n32k32). */
 int fastfp_fp64_peak(int device, int kind, int iters, double* tflops, double* ms);
 
 #ifdef __cplusplus

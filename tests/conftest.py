@@ -12,17 +12,16 @@ EPS = 2.220446049250313e-16
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; run with -m gpu)")
 
 
 @pytest.fixture(params=["auto", "fp64"])
 def sweep_path(request, monkeypatch):
     """Run a plain-Fp GPU test on both sweep kernels: "auto" = the INT8 tensor-core kernel wherever the pack can take
-    it (else the fp64 DMMA kernel), "fp64" = the DMMA kernel always. FastFp reads FASTFP_B200_PATH at construction."""
+    it (else the fp64 DMMA kernel; the library's AUTO is the DMMA kernel, so this parameter asks for "prefer-i8"),
+    "fp64" = the DMMA kernel always. FastFp reads FASTFP_B200_PATH at construction."""
     path = request.param
-    if path == "auto" and os.environ.get("FASTFP_B200_TEST_PREFER_I8"):
-        path = "prefer-i8"  # bring-up runs: exercise the tensor kernel before AUTO resolves to it
-    monkeypatch.setenv("FASTFP_B200_PATH", path)
+    monkeypatch.setenv("FASTFP_B200_PATH", "prefer-i8" if path == "auto" else path)
     return path
 
 

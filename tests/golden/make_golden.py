@@ -1,5 +1,5 @@
 """Generate the golden fixtures in this directory by executing the UNMODIFIED reference
-source (``/root/reference/fastfp/*.py``) on seeded synthetic inputs.
+source (a checkout of gabefreedman/fastfp, ``fastfp/*.py``) on seeded synthetic inputs.
 
 JAX and ``enterprise`` are not installable in the build image (no network), so the reference
 modules are imported with two stand-ins placed in ``sys.modules`` first:
@@ -11,10 +11,10 @@ modules are imported with two stand-ins placed in ``sys.modules`` first:
 * ``enterprise*`` -> empty stub modules (they are imported at the top of
   ``fastfp/utils.py`` but never touched by the hot path).
 
-Run (in the build container, where /root/reference exists):
-    python tests/golden/make_golden.py
+Run with the reference checkout named by FASTFP_REFERENCE:
+    FASTFP_REFERENCE=<path to fastfp> python tests/golden/make_golden.py
 Outputs: tests/golden/fp_white.npz, fp_red.npz, nmfp.npz  (inputs + reference outputs +
-longdouble truth), all small enough to commit. Nothing here runs on the GPU box.
+longdouble truth), all small enough to commit. Nothing here runs on the GPU.
 """
 from __future__ import annotations
 
@@ -26,7 +26,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(os.path.dirname(HERE))
-REFERENCE = os.environ.get("FASTFP_REFERENCE", "/root/reference")
+REFERENCE = os.environ.get("FASTFP_REFERENCE", "")
 
 
 # --------------------------------------------------------------------------------------
@@ -136,6 +136,8 @@ def install_shims():
 
 # --------------------------------------------------------------------------------------
 def main():
+    if not REFERENCE:
+        raise SystemExit("set FASTFP_REFERENCE to a checkout of the reference fastfp source")
     install_shims()
     sys.path.insert(0, REFERENCE)
     sys.path.insert(0, REPO)

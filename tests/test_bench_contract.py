@@ -1,5 +1,5 @@
 """bench.py's output contract on the CPU-runnable arm: exactly one JSON line on stdout (library chatter goes
-to stderr), the keys the driver reads, and the reference arm's fixed fields. The GPU arm needs a B200 and is
+to stderr), the keys the driver reads, and the reference arm's fixed fields. The GPU arm needs an H100 and is
 exercised by the driver; this guards the shared plumbing (argument handling, emit(), stdout redirection)."""
 import json
 import os

@@ -1,5 +1,5 @@
 """GPU parity tests for the plain Fp path: the CUDA sweep (through the C ABI) against the golden
-vectors of the reference source, the oracle and the longdouble truth. Run with -m gpu on a B200."""
+vectors of the reference source, the oracle and the longdouble truth. Run with -m gpu on an H100."""
 import numpy as np
 import pytest
 

@@ -1,6 +1,6 @@
 """GPU tests at the limits of the tensor-core sweep (fp_sweep_i8.cu): the widest basis and the longest pulsar it
 takes in one pass (m = 127 -> all 128 operand rows, n = 16384 -> the int32 accumulators' exactness bound), wider
-bases in row groups up to m = 639, the narrowest one, and the hand-over to the fp64 kernel just outside. Run with -m gpu on a B200."""
+bases in row groups up to m = 639, the narrowest one, and the hand-over to the fp64 kernel just outside. Run with -m gpu on an H100."""
 import numpy as np
 import pytest
 
@@ -44,12 +44,12 @@ def test_one_toa_too_many_goes_to_the_fp64_kernel_pulsar_by_pulsar():
     # kernel the other two, in the same call
     pta = synth.make_pta(3, [16385, 300, 1207], n_tm=[7, 7, 9], ncomps=60, seed=32)
     mats = (pta.Nvecs, pta.Ts, pta.sigmas)
-    assert fastfp_b200.FastFp(pta.psrs).prepare(*mats).path == "mixed"        # auto
+    assert fastfp_b200.FastFp(pta.psrs).prepare(*mats).path == "fp64"         # auto: the DMMA kernel
     assert fastfp_b200.FastFp(pta.psrs, path="prefer-i8").prepare(*mats).path == "mixed"
     with pytest.raises(_cabi.FastFpError):
         fastfp_b200.FastFp(pta.psrs, path="i8").prepare(*mats)
     freqs = np.concatenate((synth.fp_freqs(30), np.array([1.0, 17.5, 60.0]) / pta.Tspan))
-    tm, tol = _against_truth(pta, freqs, "auto", expect="mixed")
+    tm, tol = _against_truth(pta, freqs, "prefer-i8", expect="mixed")
     t64, _ = _against_truth(pta, freqs, "fp64")
     np.testing.assert_array_equal(tm[0], t64[0])            # pulsar 0 ran on the fp64 kernel: the same bits
     assert np.all(np.abs(tm - t64) <= 2 * tol)
@@ -59,7 +59,7 @@ def test_one_toa_too_many_goes_to_the_fp64_kernel_pulsar_by_pulsar():
     sigs = [RN_container(q, Ffreqs=pta.Ffreqs) for q in pta.psrs]
     samples = {k: v for k, v in synth.draw_samples(pta, 3).items() if not k.startswith("gw_")}
     fn = synth.nmfp_freqs(40, pta.Tspan) * 1.003
-    a = NMFP(pta.psrs, sigs)(fn, samples, pta.Nvecs, pta.Ts, pta.TNTs)
+    a = NMFP(pta.psrs, sigs, path="prefer-i8")(fn, samples, pta.Nvecs, pta.Ts, pta.TNTs)
     b = NMFP(pta.psrs, sigs, path="fp64")(fn, samples, pta.Nvecs, pta.Ts, pta.TNTs)
     np.testing.assert_allclose(a, b, rtol=1e-6)
 
