@@ -237,164 +237,111 @@ class Pack:
                 "reference's general LU solve is only available through get_xCy.", RuntimeWarning, stacklevel=3)
 
     @classmethod
-    def create_fp(cls, toas, residuals, Nvecs, Ts, sigmas, device: int = 0, stream: int = 0) -> "Pack":
-        P, n, m, toas, residuals, Nvecs, Ts, sigmas = _check_lists(toas, residuals, Nvecs, Ts, sigmas, "sigmas")
-        lib = load()
-        require_device()
-        h = C.c_void_p()
-        check(
-            lib.fastfp_pack_create(
-                device, P, _int64_array(n), _int64_array(m), _ptr_array(toas), _ptr_array(residuals),
-                _ptr_array(Nvecs), _ptr_array(Ts), _ptr_array(sigmas), C.c_void_p(stream), C.byref(h),
-            )
-        )
-        return cls(h, P, device, False, n, m)
-
-    @classmethod
-    def create_nmfp(cls, toas, residuals, Nvecs, Ts, TNTs, m_fix, phiinv_fix, device: int = 0, stream: int = 0):
-        P, n, m, toas, residuals, Nvecs, Ts, TNTs = _check_lists(toas, residuals, Nvecs, Ts, TNTs, "TNTs")
-        if len(m_fix) != P or len(phiinv_fix) != P:
-            raise ValueError("m_fix and phiinv_fix must have one entry per pulsar")
-        pf = []
-        for p in range(P):
-            if not 0 <= int(m_fix[p]) <= m[p]:
-                raise ValueError(f"pulsar {p}: m_fix out of range")
-            a = as_f64(phiinv_fix[p]).reshape(-1)
-            if a.shape[0] != int(m_fix[p]):
-                raise ValueError(f"pulsar {p}: phiinv_fix must have m_fix entries")
-            pf.append(a if a.size else np.zeros(1))
-        lib = load()
-        require_device()
-        h = C.c_void_p()
-        check(
-            lib.fastfp_nmfp_pack_create(
-                device, P, _int64_array(n), _int64_array(m), _ptr_array(toas), _ptr_array(residuals),
-                _ptr_array(Nvecs), _ptr_array(Ts), _ptr_array(TNTs), _int64_array(m_fix), _ptr_array(pf),
-                C.c_void_p(stream), C.byref(h),
-            )
-        )
-        return cls(h, P, device, True, n, m)
-
-    @classmethod
-    def create_blockn(cls, toas, residuals, Nvecs, Ts, mats, m_fix=None, phiinv_fix=None, device: int = 0,
-                      stream: int = 0) -> "Pack":
-        """Pack with a block-diagonal N (kernel ECORR) for at least one pulsar. ``mats`` are the
-        sigmas (plain Fp, ``m_fix is None``) or the TNTs (nmfp), formed with the block N."""
+    def create(cls, toas, residuals, Nvecs, Ts, mats, m_fix=None, phiinv_fix=None, device: int = 0,
+               stream: int = 0) -> "Pack":
+        """Pack the pulsar lists on ``device``. ``mats`` are the sigmas of a plain-Fp pack (``m_fix is None``) or the
+        TNTs of an nmfp pack, whose ``m_fix[p]`` leading columns are draw-independent with prior ``phiinv_fix[p]``.
+        A ``blockn`` object among the ``Nvecs`` (a block-diagonal N, kernel ECORR) makes the pack a block-N one."""
         from . import blockn
 
-        P = len(toas)
-        if P < 1 or not (len(residuals) == len(Nvecs) == len(Ts) == len(mats) == P):
-            raise ValueError("toas, residuals, Nvecs, Ts and the matrices must be lists of equal length P >= 1")
-        Ts = [as_f64(T) for T in Ts]
-        mats = [as_f64(a) for a in mats]
-        prep, n, m = [], [], []
+        block = any(blockn.is_block(N) for N in Nvecs)
+        if block:
+            P = len(toas)
+            if P < 1 or not (len(residuals) == len(Nvecs) == len(Ts) == len(mats) == P):
+                raise ValueError("toas, residuals, Nvecs, Ts and the matrices must be lists of equal length P >= 1")
+            Ts, mats = [as_f64(T) for T in Ts], [as_f64(a) for a in mats]
+            prep, n, m = [], [], []
+            for p in range(P):
+                if Ts[p].ndim != 2 or mats[p].shape != (Ts[p].shape[1],) * 2:
+                    raise ValueError(f"pulsar {p}: Ts must be (ntoa, nbasis) and the matrix (nbasis, nbasis)")
+                ci = load().fastfp_sweep_chunk_toas(Ts[p].shape[1], 1)
+                if ci <= 0:
+                    raise ValueError(f"pulsar {p}: basis width {Ts[p].shape[1]} is not supported with a block-diagonal N")
+                prep.append(blockn.prepare(toas[p], residuals[p], Nvecs[p], Ts[p], ci))
+                n.append(prep[-1]["toas"].shape[0])
+                m.append(Ts[p].shape[1])
+        else:
+            what = "sigmas" if m_fix is None else "TNTs"
+            P, n, m, toas, residuals, Nvecs, Ts, mats = _check_lists(toas, residuals, Nvecs, Ts, mats, what)
+        nmfp, fixed = m_fix is not None, (None, None)
+        if nmfp:
+            if len(m_fix) != P or len(phiinv_fix) != P:
+                raise ValueError("m_fix and phiinv_fix must have one entry per pulsar")
+            pf = []
+            for p in range(P):
+                if not 0 <= int(m_fix[p]) <= m[p]:
+                    raise ValueError(f"pulsar {p}: m_fix out of range")
+                a = as_f64(phiinv_fix[p]).reshape(-1)
+                if a.shape[0] != int(m_fix[p]):
+                    raise ValueError(f"pulsar {p}: phiinv_fix must have m_fix entries")
+                pf.append(a if a.size else np.zeros(1))
+            fixed = (_int64_array(m_fix), _ptr_array(pf))
         lib = load()
-        for p in range(P):
-            if Ts[p].ndim != 2 or mats[p].shape != (Ts[p].shape[1],) * 2:
-                raise ValueError(f"pulsar {p}: Ts must be (ntoa, nbasis) and the matrix (nbasis, nbasis)")
-            ci = lib.fastfp_sweep_chunk_toas(Ts[p].shape[1], 1)
-            if ci <= 0:
-                raise ValueError(f"pulsar {p}: basis width {Ts[p].shape[1]} is not supported with a block-diagonal N")
-            d = blockn.prepare(toas[p], residuals[p], Nvecs[p], Ts[p], ci)
-            prep.append(d)
-            n.append(d["toas"].shape[0])
-            m.append(Ts[p].shape[1])
         require_device()
-        pf = None
-        if m_fix is not None:
-            pf = [as_f64(a).reshape(-1) if len(a) else np.zeros(1) for a in phiinv_fix]
-        i32pp = (C.POINTER(C.c_int32) * P)(*[d["slot_idx"].ctypes.data_as(C.POINTER(C.c_int32)) for d in prep])
-        u8pp = (C.POINTER(C.c_ubyte) * P)(*[d["done_mask"].ctypes.data_as(C.POINTER(C.c_ubyte)) for d in prep])
         h = C.c_void_p()
-        check(
-            lib.fastfp_pack_create_blockn(
-                device, P, _int64_array(n), _int64_array(m), _ptr_array([d["toas"] for d in prep]),
-                _ptr_array([d["res"] for d in prep]), _ptr_array([d["res_w"] for d in prep]),
-                _ptr_array([d["Nvec"] for d in prep]), _ptr_array([d["T"] for d in prep]), _ptr_array(mats),
-                i32pp, _ptr_array([d["slot_val"] for d in prep]), u8pp,
-                _int64_array(m_fix) if m_fix is not None else None, _ptr_array(pf) if pf is not None else None,
-                C.c_void_p(stream), C.byref(h),
-            )
-        )
-        return cls(h, P, device, m_fix is not None, n, m)
+        head = (device, P, _int64_array(n), _int64_array(m))
+        tail = (C.c_void_p(stream), C.byref(h))
+        if block:
+            i32pp = (C.POINTER(C.c_int32) * P)(*[d["slot_idx"].ctypes.data_as(C.POINTER(C.c_int32)) for d in prep])
+            u8pp = (C.POINTER(C.c_ubyte) * P)(*[d["done_mask"].ctypes.data_as(C.POINTER(C.c_ubyte)) for d in prep])
+            arrays = [_ptr_array([d[k] for d in prep]) for k in ("toas", "res", "res_w", "Nvec", "T")]
+            check(lib.fastfp_pack_create_blockn(*head, *arrays, _ptr_array(mats), i32pp,
+                                                _ptr_array([d["slot_val"] for d in prep]), u8pp,
+                                                *fixed, *tail))
+        elif nmfp:
+            check(lib.fastfp_nmfp_pack_create(*head, *map(_ptr_array, (toas, residuals, Nvecs, Ts, mats)), *fixed, *tail))
+        else:
+            check(lib.fastfp_pack_create(*head, *map(_ptr_array, (toas, residuals, Nvecs, Ts, mats)), *tail))
+        return cls(h, P, device, nmfp, n, m)
 
     # -- sweeps -------------------------------------------------------------------------
-    def fp_sweep(self, freqs, out=None, stream: int = 0, terms: bool = False):
-        """``freqs``: host ndarray or ``(device_address, F)``; ``out``: None (a host array is
-        returned), a host ndarray, or an integer device address."""
-        lib = load()
+    @staticmethod
+    def _stage(freqs, out, rows=None):
+        """``freqs``: host ndarray or ``(device_address, F)``; ``out``: None (a host array of shape ``(F,)`` or
+        ``(rows, F)`` is allocated and returned), a host ndarray, or an integer device address. Returns the frequency
+        and output arguments (kept alive by the caller), ``F``, the array to return and the location flags."""
         flags = 0
         if isinstance(freqs, tuple):
-            fptr, F = freqs
+            freqs, F = freqs
             flags |= FREQS_ON_DEVICE
         else:
             freqs = as_f64(freqs).reshape(-1)
-            fptr, F = freqs, freqs.shape[0]
+            F = freqs.shape[0]
         ret = None
         if out is None:
-            ret = np.empty((self.P, F) if terms else (F,), dtype=np.float64)
-            optr = ret
-        elif isinstance(out, np.ndarray):
-            optr = out
-        else:
-            optr = out
+            out = ret = np.empty((F,) if rows is None else (rows, F), dtype=np.float64)
+        elif not isinstance(out, np.ndarray):
             flags |= OUT_ON_DEVICE
-        fn = lib.fastfp_fp_terms if terms else lib.fastfp_fp_sweep
-        check(fn(self._h, _vp(fptr), F, _vp(optr), flags, C.c_void_p(stream)))
+        return freqs, out, F, ret, flags
+
+    def fp_sweep(self, freqs, out=None, stream: int = 0, terms: bool = False):
+        """``freqs``: host ndarray or ``(device_address, F)``; ``out``: None (a host array is
+        returned), a host ndarray, or an integer device address."""
+        freqs, out, F, ret, flags = self._stage(freqs, out, self.P if terms else None)
+        fn = load().fastfp_fp_terms if terms else load().fastfp_fp_sweep
+        check(fn(self._h, _vp(freqs), F, _vp(out), flags, C.c_void_p(stream)))
         return ret
 
     def fe_sweep(self, freqs, fplus, fcross, out=None, stream: int = 0):
         """Fe-statistic for ``S`` sky positions: ``fplus``, ``fcross`` host arrays ``(S, P)``; returns / fills
         ``(S, F)``. ``freqs`` / ``out`` as in :meth:`fp_sweep`."""
-        lib = load()
         fplus, fcross = as_f64(fplus), as_f64(fcross)
         if fplus.ndim != 2 or fplus.shape != fcross.shape or fplus.shape[1] != self.P:
             raise ValueError("fplus and fcross must both have shape (n_sky, n_pulsars)")
         S = fplus.shape[0]
-        flags = 0
-        if isinstance(freqs, tuple):
-            fptr, F = freqs
-            flags |= FREQS_ON_DEVICE
-        else:
-            freqs = as_f64(freqs).reshape(-1)
-            fptr, F = freqs, freqs.shape[0]
-        ret = None
-        if out is None:
-            ret = np.empty((S, F), dtype=np.float64)
-            optr = ret
-        elif isinstance(out, np.ndarray):
-            optr = out
-        else:
-            optr = out
-            flags |= OUT_ON_DEVICE
-        check(lib.fastfp_fe_sweep(self._h, _vp(fptr), F, _vp(fplus), _vp(fcross), S, _vp(optr), flags, C.c_void_p(stream)))
+        freqs, out, F, ret, flags = self._stage(freqs, out, S)
+        check(load().fastfp_fe_sweep(self._h, _vp(freqs), F, _vp(fplus), _vp(fcross), S, _vp(out), flags,
+                                     C.c_void_p(stream)))
         return ret
 
     def nmfp_sweep(self, freqs, phiinv_var, D: int, out=None, stream: int = 0):
-        lib = load()
-        flags = 0
-        if isinstance(freqs, tuple):
-            fptr, F = freqs
-            flags |= FREQS_ON_DEVICE
-        else:
-            freqs = as_f64(freqs).reshape(-1)
-            fptr, F = freqs, freqs.shape[0]
+        freqs, out, F, ret, flags = self._stage(freqs, out, D)
         if isinstance(phiinv_var, np.ndarray):
             phiinv_var = as_f64(phiinv_var)
-            pptr = phiinv_var
         else:
-            pptr = phiinv_var
             flags |= PARAMS_ON_DEVICE
-        ret = None
-        if out is None:
-            ret = np.empty((D, F), dtype=np.float64)
-            optr = ret
-        elif isinstance(out, np.ndarray):
-            optr = out
-        else:
-            optr = out
-            flags |= OUT_ON_DEVICE
-        check(lib.fastfp_nmfp_sweep(self._h, _vp(fptr), F, _vp(pptr), D, _vp(optr), flags, C.c_void_p(stream)))
+        check(load().fastfp_nmfp_sweep(self._h, _vp(freqs), F, _vp(phiinv_var), D, _vp(out), flags,
+                                       C.c_void_p(stream)))
         return ret
 
     # the two halves of nmfp_sweep as separate calls (device pointers only): parallel.py shards them in two dimensions

@@ -45,14 +45,6 @@ int powerlaw_phiinv_impl(const fastfp_pack* pk, const double* const* Ffreqs, con
                          const double* curn_log10_A, const double* curn_gamma, double* out,
                          cudaStream_t st);
 
-// Common part of the two pack constructors: validate, lay out, upload the raw arrays.
-struct Staging {
-  double *d_toas = nullptr, *d_res = nullptr, *d_Nvec = nullptr, *d_T = nullptr;
-  ~Staging() {
-    cudaFree(d_toas); cudaFree(d_res); cudaFree(d_Nvec); cudaFree(d_T);
-  }
-};
-
 static int pack_layout(fastfp_pack* pk, int P, const int64_t* n, const int64_t* m,
                        const int64_t* m_fix, const double* const* toas, bool blockn = false) {
   pk->P = P;
@@ -135,22 +127,30 @@ static int pack_layout(fastfp_pack* pk, int P, const int64_t* n, const int64_t* 
   return 0;
 }
 
-static int upload_ragged(double** dst, const double* const* src, const fastfp_pack* pk, int which,
-                         cudaStream_t st) {
-  // which: 0 = length n_p, 1 = n_p*m_p (T), 2 = m_p*m_p
-  int64_t total = 0;
-  for (auto& pm : pk->meta)
-    total += which == 0 ? pm.n : which == 1 ? (int64_t)pm.n * pm.m : (int64_t)pm.m * pm.m;
-  if (*dst == nullptr) FFP_CUDA(cudaMalloc(dst, (size_t)total * 8));
+// which: 0 = length n_p, 1 = n_p*m_p (T), 2 = m_p*m_p
+static int64_t ragged_count(const PulsarMeta& pm, int which) {
+  return which == 0 ? pm.n : which == 1 ? (int64_t)pm.n * pm.m : (int64_t)pm.m * pm.m;
+}
+
+// the per-pulsar arrays src[p] back to back into dst
+static int upload_ragged(double* dst, const double* const* src, const fastfp_pack* pk, int which, cudaStream_t st) {
   int64_t off = 0;
   for (int p = 0; p < pk->P; ++p) {
-    const PulsarMeta& pm = pk->meta[p];
-    const int64_t cnt = which == 0 ? pm.n : which == 1 ? (int64_t)pm.n * pm.m : (int64_t)pm.m * pm.m;
+    const int64_t cnt = ragged_count(pk->meta[p], which);
     if (!src[p]) { set_error("null per-pulsar array"); return FASTFP_ERR_INVALID; }
-    FFP_CUDA(cudaMemcpyAsync(*dst + off, src[p], (size_t)cnt * 8, cudaMemcpyHostToDevice, st));
+    FFP_CUDA(cudaMemcpyAsync(dst + off, src[p], (size_t)cnt * 8, cudaMemcpyHostToDevice, st));
     off += cnt;
   }
   return 0;
+}
+
+// upload_ragged into a new staging buffer
+static int stage_ragged(DeviceBuf<double>* dst, const double* const* src, const fastfp_pack* pk, int which,
+                        cudaStream_t st) {
+  int64_t total = 0;
+  for (auto& pm : pk->meta) total += ragged_count(pm, which);
+  FFP_CUDA(dev_alloc(dst, (size_t)total));
+  return upload_ragged(dst->get(), src, pk, which, st);
 }
 
 // sum_i 1/N_i per pulsar in extended precision (the tensor sweep derives c N^-1 c from s N^-1 s with it)
@@ -175,6 +175,110 @@ static void pack_free(fastfp_pack* pk) {
   delete pk;
 }
 
+struct BlockNHost {  // host side arrays of a block-diagonal N (fastfp_pack_create_blockn)
+  const double* const* res_w;
+  const int32_t* const* slot_idx;
+  const double* const* slot_val;
+  const unsigned char* const* done_mask;
+};
+
+// block-N slot indices into a new staging buffer, the per-chunk slot masks into the pack
+static int stage_slots(fastfp_pack* pk, const BlockNHost& bn, DeviceBuf<int>* d_sidx, cudaStream_t st) {
+  int64_t ntot = 0, nchtot = 0;
+  for (auto& pm : pk->meta) { ntot += pm.n; nchtot += pm.nch; }
+  FFP_CUDA(dev_alloc(d_sidx, (size_t)ntot));
+  FFP_CUDA(cudaMalloc(&pk->d_done_mask, (size_t)nchtot));
+  for (int p = 0; p < pk->P; ++p) {
+    const PulsarMeta& pm = pk->meta[p];
+    if (!bn.slot_idx[p] || !bn.done_mask[p]) { set_error("null slot array"); return FASTFP_ERR_INVALID; }
+    FFP_CUDA(cudaMemcpyAsync(d_sidx->get() + pm.raw_off, bn.slot_idx[p], (size_t)pm.n * sizeof(int),
+                             cudaMemcpyHostToDevice, st));
+    FFP_CUDA(cudaMemcpyAsync(pk->d_done_mask + pm.dm_off, bn.done_mask[p], (size_t)pm.nch, cudaMemcpyHostToDevice, st));
+  }
+  return 0;
+}
+
+// The one pack builder behind the three constructors. mats are the sigmas of a plain-Fp pack (m_fix null) or the TNTs
+// of an nmfp pack (m_fix / phiinv_fix: the draw-independent leading columns and their prior). bn null: diagonal N.
+static int build_pack(int device, int P, const int64_t* n, const int64_t* m, const double* const* toas,
+                      const double* const* residuals, const double* const* Nvecs, const double* const* Ts,
+                      const double* const* mats, const int64_t* m_fix, const double* const* phiinv_fix,
+                      const BlockNHost* bn, void* stream, fastfp_pack_t** out) {
+  *out = nullptr;
+  DeviceGuard g(device);
+  if (!g.ok) { set_error("cannot select CUDA device " + std::to_string(device)); return FASTFP_ERR_CUDA; }
+  cudaStream_t st = (cudaStream_t)stream;
+  fastfp_pack* pk = new fastfp_pack();
+  pk->device = device;
+  pk->nmfp = m_fix != nullptr;
+  int rc = pack_layout(pk, P, n, m, m_fix, toas, bn != nullptr);
+  DeviceBuf<double> d_toas, d_res, d_Nvec, d_T, d_mat, d_pf, d_resw, d_sval;
+  DeviceBuf<int> d_sidx;
+  if (!rc) rc = stage_ragged(&d_toas, toas, pk, 0, st);
+  if (!rc) rc = stage_ragged(&d_res, residuals, pk, 0, st);
+  if (!rc) rc = stage_ragged(&d_Nvec, Nvecs, pk, 0, st);
+  if (!rc) rc = stage_ragged(&d_T, Ts, pk, 1, st);
+  if (!rc && bn) rc = stage_ragged(&d_resw, bn->res_w, pk, 0, st);
+  if (!rc && bn) rc = stage_ragged(&d_sval, bn->slot_val, pk, 0, st);
+  if (!rc && bn) rc = stage_slots(pk, *bn, &d_sidx, st);
+  const BlockNDev bnd{d_resw.get(), d_sidx.get(), d_sval.get()};
+  const BlockNDev* bnp = bn ? &bnd : nullptr;
+  if (!rc && !bn) set_ninv_sums(pk, Nvecs);  // only the tensor sweep reads them, and it takes no block-N pack
+  if (!rc && !pk->nmfp) {
+    rc = upload_ragged(pk->d_L, mats, pk, 2, st);  // sigmas, into the factor buffer pack_layout allocated
+    if (!rc) rc = launch_fp_precompute(pk, d_toas.get(), d_res.get(), d_Nvec.get(), d_T.get(), st, nullptr, bnp);
+    if (!rc) rc = build_i8_planes(pk, st);  // digit planes for the pulsars the tensor sweep takes (none with block-N)
+  } else if (!rc) {
+    rc = stage_ragged(&d_mat, mats, pk, 2, st);  // TNTs
+    if (!rc) {
+      // fixed phiinv: (P, MAX_M) padded
+      std::vector<double> pf((size_t)P * MAX_M, 0.0);
+      for (int p = 0; p < P; ++p)
+        for (int j = 0; j < pk->meta[p].mfix; ++j) pf[(size_t)p * MAX_M + j] = phiinv_fix[p][j];
+      cudaError_t e = dev_alloc(&d_pf, pf.size());
+      if (e == cudaSuccess) e = cudaMemcpy(d_pf.get(), pf.data(), pf.size() * 8, cudaMemcpyHostToDevice);
+      if (e != cudaSuccess) rc = cuda_fail(e, "upload phiinv_fix");
+    }
+    if (!rc) rc = nmfp_pack_finish(pk, d_toas.get(), d_res.get(), d_Nvec.get(), d_T.get(), d_mat.get(), d_pf.get(), st, bnp);
+  }
+  cudaStreamSynchronize(st);  // the staging buffers are released on return, after the work that reads them
+  if (rc) { pack_free(pk); return rc; }
+  *out = pk;
+  return FASTFP_OK;
+}
+
+// The start of every call that runs work on a pack. While it lives the pack's device is current; select() reports
+// FASTFP_ERR_CUDA if it could not be made so. stage() also resolves the device addresses of the F frequencies (the
+// caller's pointer, or the host array copied into pk->d_freqs) and of the nout result doubles (the caller's pointer,
+// or the pack-owned buffer *buf that the caller copies back to host memory).
+struct PackCall {
+  const fastfp_pack* pk;
+  cudaStream_t st;
+  DeviceGuard dev;
+  PackCall(const fastfp_pack* p, void* stream) : pk(p), st((cudaStream_t)stream), dev(p->device) {}
+  int select() const {
+    if (dev.ok) return FASTFP_OK;
+    set_error("cannot select CUDA device " + std::to_string(pk->device));
+    return FASTFP_ERR_CUDA;
+  }
+  int stage(const double* freqs, int64_t F, double* out, int64_t nout, int flags, const double** d_freqs,
+            double** d_out, double** buf, int64_t* cap) const {
+    if (int rc = select()) return rc;
+    *d_freqs = freqs;
+    if (!(flags & FASTFP_FREQS_ON_DEVICE)) {
+      if (int rc = ensure(&pk->d_freqs, &pk->freqs_cap, F)) return rc;
+      FFP_CUDA(cudaMemcpyAsync(pk->d_freqs, freqs, (size_t)F * 8, cudaMemcpyHostToDevice, st));
+      *d_freqs = pk->d_freqs;
+    }
+    *d_out = out;
+    if (!(flags & FASTFP_OUT_ON_DEVICE)) {
+      if (int rc = ensure(buf, cap, nout)) return rc;
+      *d_out = *buf;
+    }
+    return FASTFP_OK;
+  }
+};
+
 }  // namespace ffp
 
 using namespace ffp;
@@ -198,27 +302,7 @@ int fastfp_pack_create(int device, int P, const int64_t* n, const int64_t* m,
     set_error("fastfp_pack_create: null argument or P < 1");
     return FASTFP_ERR_INVALID;
   }
-  *out = nullptr;
-  DeviceGuard g(device);
-  if (!g.ok) { set_error("cannot select CUDA device " + std::to_string(device)); return FASTFP_ERR_CUDA; }
-  cudaStream_t st = (cudaStream_t)stream;
-  fastfp_pack* pk = new fastfp_pack();
-  pk->device = device;
-  int rc = pack_layout(pk, P, n, m, nullptr, toas);
-  Staging sg;
-  if (!rc) rc = upload_ragged(&sg.d_toas, toas, pk, 0, st);
-  if (!rc) rc = upload_ragged(&sg.d_res, residuals, pk, 0, st);
-  if (!rc) rc = upload_ragged(&sg.d_Nvec, Nvecs, pk, 0, st);
-  if (!rc) rc = upload_ragged(&sg.d_T, Ts, pk, 1, st);
-  if (!rc) rc = upload_ragged(&pk->d_L, sigmas, pk, 2, st);
-  if (!rc) rc = launch_fp_precompute(pk, sg.d_toas, sg.d_res, sg.d_Nvec, sg.d_T, st);
-  if (!rc) {
-    set_ninv_sums(pk, Nvecs);
-    rc = build_i8_planes(pk, st);  // digit planes for the tensor path when every pulsar fits its tile
-  }
-  if (rc) { pack_free(pk); return rc; }
-  *out = pk;
-  return FASTFP_OK;
+  return build_pack(device, P, n, m, toas, residuals, Nvecs, Ts, sigmas, nullptr, nullptr, nullptr, stream, out);
 }
 
 int fastfp_pack_set_path(fastfp_pack_t* pk, int path) {
@@ -254,37 +338,7 @@ int fastfp_nmfp_pack_create(int device, int P, const int64_t* n, const int64_t* 
     set_error("fastfp_nmfp_pack_create: null argument or P < 1");
     return FASTFP_ERR_INVALID;
   }
-  *out = nullptr;
-  DeviceGuard g(device);
-  if (!g.ok) { set_error("cannot select CUDA device " + std::to_string(device)); return FASTFP_ERR_CUDA; }
-  cudaStream_t st = (cudaStream_t)stream;
-  fastfp_pack* pk = new fastfp_pack();
-  pk->device = device;
-  pk->nmfp = true;
-  int rc = pack_layout(pk, P, n, m, m_fix, toas);
-  Staging sg;
-  double *d_TNT = nullptr, *d_pf = nullptr;
-  if (!rc) rc = upload_ragged(&sg.d_toas, toas, pk, 0, st);
-  if (!rc) rc = upload_ragged(&sg.d_res, residuals, pk, 0, st);
-  if (!rc) rc = upload_ragged(&sg.d_Nvec, Nvecs, pk, 0, st);
-  if (!rc) rc = upload_ragged(&sg.d_T, Ts, pk, 1, st);
-  if (!rc) rc = upload_ragged(&d_TNT, TNTs, pk, 2, st);
-  if (!rc) {
-    // fixed phiinv: (P, MAX_M) padded
-    std::vector<double> pf((size_t)P * MAX_M, 0.0);
-    for (int p = 0; p < P; ++p)
-      for (int j = 0; j < pk->meta[p].mfix; ++j) pf[(size_t)p * MAX_M + j] = phiinv_fix[p][j];
-    cudaError_t e = cudaMalloc(&d_pf, pf.size() * 8);
-    if (e == cudaSuccess) e = cudaMemcpy(d_pf, pf.data(), pf.size() * 8, cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) rc = cuda_fail(e, "upload phiinv_fix");
-  }
-  if (!rc) set_ninv_sums(pk, Nvecs);
-  if (!rc) rc = nmfp_pack_finish(pk, sg.d_toas, sg.d_res, sg.d_Nvec, sg.d_T, d_TNT, d_pf, st);
-  cudaFree(d_TNT);
-  cudaFree(d_pf);
-  if (rc) { pack_free(pk); return rc; }
-  *out = pk;
-  return FASTFP_OK;
+  return build_pack(device, P, n, m, toas, residuals, Nvecs, Ts, TNTs, m_fix, phiinv_fix, nullptr, stream, out);
 }
 
 int fastfp_sweep_chunk_toas(int64_t m, int blockn) {
@@ -306,58 +360,8 @@ int fastfp_pack_create_blockn(int device, int P, const int64_t* n, const int64_t
     set_error("fastfp_pack_create_blockn: null argument or P < 1");
     return FASTFP_ERR_INVALID;
   }
-  *out = nullptr;
-  DeviceGuard g(device);
-  if (!g.ok) { set_error("cannot select CUDA device " + std::to_string(device)); return FASTFP_ERR_CUDA; }
-  cudaStream_t st = (cudaStream_t)stream;
-  fastfp_pack* pk = new fastfp_pack();
-  pk->device = device;
-  pk->nmfp = m_fix != nullptr;
-  int rc = pack_layout(pk, P, n, m, m_fix, toas, true);
-  Staging sg;
-  double *d_resw = nullptr, *d_sval = nullptr, *d_mat = nullptr, *d_pf = nullptr;
-  int* d_sidx = nullptr;
-  if (!rc) rc = upload_ragged(&sg.d_toas, toas, pk, 0, st);
-  if (!rc) rc = upload_ragged(&sg.d_res, residuals, pk, 0, st);
-  if (!rc) rc = upload_ragged(&d_resw, residuals_w, pk, 0, st);
-  if (!rc) rc = upload_ragged(&sg.d_Nvec, Nvecs, pk, 0, st);
-  if (!rc) rc = upload_ragged(&sg.d_T, Ts, pk, 1, st);
-  if (!rc) rc = upload_ragged(&d_sval, slot_val, pk, 0, st);
-  if (!rc) {
-    int64_t ntot = 0, nchtot = 0;
-    for (auto& pm : pk->meta) { ntot += pm.n; nchtot += pm.nch; }
-    cudaError_t e = cudaMalloc(&d_sidx, (size_t)ntot * sizeof(int));
-    if (e == cudaSuccess) e = cudaMalloc(&pk->d_done_mask, (size_t)nchtot);
-    for (int p = 0; p < P && e == cudaSuccess; ++p) {
-      const PulsarMeta& pm = pk->meta[p];
-      if (!slot_idx[p] || !done_mask[p]) { rc = FASTFP_ERR_INVALID; set_error("null slot array"); break; }
-      e = cudaMemcpyAsync(d_sidx + pm.raw_off, slot_idx[p], (size_t)pm.n * sizeof(int), cudaMemcpyHostToDevice, st);
-      if (e == cudaSuccess)
-        e = cudaMemcpyAsync(pk->d_done_mask + pm.dm_off, done_mask[p], (size_t)pm.nch, cudaMemcpyHostToDevice, st);
-    }
-    if (e != cudaSuccess) rc = cuda_fail(e, "block-N side arrays");
-  }
-  BlockNDev bn{d_resw, d_sidx, d_sval};
-  if (!rc && !pk->nmfp) {
-    rc = upload_ragged(&pk->d_L, mats, pk, 2, st);  // sigmas
-    if (!rc) rc = launch_fp_precompute(pk, sg.d_toas, sg.d_res, sg.d_Nvec, sg.d_T, st, nullptr, &bn);
-  } else if (!rc) {
-    rc = upload_ragged(&d_mat, mats, pk, 2, st);  // TNTs
-    if (!rc) {
-      std::vector<double> pf((size_t)P * MAX_M, 0.0);
-      for (int p = 0; p < P; ++p)
-        for (int j = 0; j < pk->meta[p].mfix; ++j) pf[(size_t)p * MAX_M + j] = phiinv_fix[p][j];
-      cudaError_t e = cudaMalloc(&d_pf, pf.size() * 8);
-      if (e == cudaSuccess) e = cudaMemcpy(d_pf, pf.data(), pf.size() * 8, cudaMemcpyHostToDevice);
-      if (e != cudaSuccess) rc = cuda_fail(e, "upload phiinv_fix");
-    }
-    if (!rc) rc = nmfp_pack_finish(pk, sg.d_toas, sg.d_res, sg.d_Nvec, sg.d_T, d_mat, d_pf, st, &bn);
-  }
-  cudaStreamSynchronize(st);
-  cudaFree(d_resw); cudaFree(d_sval); cudaFree(d_sidx); cudaFree(d_mat); cudaFree(d_pf);
-  if (rc) { pack_free(pk); return rc; }
-  *out = pk;
-  return FASTFP_OK;
+  const BlockNHost bn{residuals_w, slot_idx, slot_val, done_mask};
+  return build_pack(device, P, n, m, toas, residuals, Nvecs, Ts, mats, m_fix, phiinv_fix, &bn, stream, out);
 }
 
 void fastfp_pack_destroy(fastfp_pack_t* pack) { pack_free(pack); }
@@ -378,12 +382,6 @@ int fastfp_pack_factor_info(const fastfp_pack_t* pack, int32_t* info) {
 // Frequencies are processed in batches so the (P, F_batch) term buffer stays bounded.
 static const int64_t kTermBudgetDoubles = 1LL << 27;  // 1 GiB
 
-// per-pulsar terms of one frequency batch on the path the pack is set to
-static int sweep_terms(const fastfp_pack* pk, const double* d_freqs, int64_t F, double* d_terms, cudaStream_t st,
-                       double* d_inner = nullptr) {
-  return launch_sweep(pk, d_freqs, F, d_terms, st, nullptr, d_inner);
-}
-
 static int fp_run(const fastfp_pack* pk, const double* freqs, int64_t F, double* out, int flags,
                   void* stream, bool want_terms) {
   if (!pk || (F > 0 && (!freqs || !out)) || F < 0) {
@@ -392,44 +390,28 @@ static int fp_run(const fastfp_pack* pk, const double* freqs, int64_t F, double*
   }
   if (pk->nmfp) { set_error("this pack was built for nmfp; use fastfp_nmfp_sweep"); return FASTFP_ERR_INVALID; }
   if (F == 0) return FASTFP_OK;
-  DeviceGuard g(pk->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  const bool fdev = flags & FASTFP_FREQS_ON_DEVICE, odev = flags & FASTFP_OUT_ON_DEVICE;
-  const double* d_freqs = freqs;
-  if (!fdev) {
-    if (int rc = ensure(&pk->d_freqs, &pk->freqs_cap, F)) return rc;
-    FFP_CUDA(cudaMemcpyAsync(pk->d_freqs, freqs, (size_t)F * 8, cudaMemcpyHostToDevice, st));
-    d_freqs = pk->d_freqs;
-  }
   const int P = pk->P;
+  const int64_t nout = want_terms ? (int64_t)P * F : F;
+  PackCall c(pk, stream);
+  const double* d_freqs;
+  double* d_out;
+  if (int rc = c.stage(freqs, F, out, nout, flags, &d_freqs, &d_out, want_terms ? &pk->d_terms : &pk->d_out,
+                       want_terms ? &pk->terms_cap : &pk->out_cap))
+    return rc;
   if (want_terms) {
-    double* d_terms = out;
-    if (!odev) {
-      if (int rc = ensure(&pk->d_terms, &pk->terms_cap, (int64_t)P * F)) return rc;
-      d_terms = pk->d_terms;
+    if (int rc = launch_sweep(pk, d_freqs, F, d_out, c.st)) return rc;
+  } else {
+    const int64_t FB = std::max<int64_t>(1024, std::min<int64_t>(F, kTermBudgetDoubles / P));
+    if (int rc = ensure(&pk->d_terms, &pk->terms_cap, (int64_t)P * std::min(FB, F))) return rc;
+    for (int64_t lo = 0; lo < F; lo += FB) {
+      const int64_t fb = std::min(FB, F - lo);
+      if (int rc = launch_sweep(pk, d_freqs + lo, fb, pk->d_terms, c.st)) return rc;
+      if (int rc = launch_reduce_terms(pk->d_terms, P, fb, d_out + lo, c.st)) return rc;
     }
-    if (int rc = sweep_terms(pk, d_freqs, F, d_terms, st)) return rc;
-    if (!odev) {
-      FFP_CUDA(cudaMemcpyAsync(out, d_terms, (size_t)P * F * 8, cudaMemcpyDeviceToHost, st));
-      FFP_CUDA(cudaStreamSynchronize(st));
-    }
-    return FASTFP_OK;
   }
-  double* d_out = out;
-  if (!odev) {
-    if (int rc = ensure(&pk->d_out, &pk->out_cap, F)) return rc;
-    d_out = pk->d_out;
-  }
-  const int64_t FB = std::max<int64_t>(1024, std::min<int64_t>(F, kTermBudgetDoubles / P));
-  if (int rc = ensure(&pk->d_terms, &pk->terms_cap, (int64_t)P * std::min(FB, F))) return rc;
-  for (int64_t lo = 0; lo < F; lo += FB) {
-    const int64_t fb = std::min(FB, F - lo);
-    if (int rc = sweep_terms(pk, d_freqs + lo, fb, pk->d_terms, st)) return rc;
-    if (int rc = launch_reduce_terms(pk->d_terms, P, fb, d_out + lo, st)) return rc;
-  }
-  if (!odev) {
-    FFP_CUDA(cudaMemcpyAsync(out, d_out, (size_t)F * 8, cudaMemcpyDeviceToHost, st));
-    FFP_CUDA(cudaStreamSynchronize(st));
+  if (!(flags & FASTFP_OUT_ON_DEVICE)) {
+    FFP_CUDA(cudaMemcpyAsync(out, d_out, (size_t)nout * 8, cudaMemcpyDeviceToHost, c.st));
+    FFP_CUDA(cudaStreamSynchronize(c.st));
   }
   return FASTFP_OK;
 }
@@ -452,38 +434,28 @@ int fastfp_fe_sweep(const fastfp_pack_t* pk, const double* freqs, int64_t F, con
   }
   if (pk->nmfp) { set_error("fastfp_fe_sweep needs a plain-Fp pack (fastfp_pack_create)"); return FASTFP_ERR_INVALID; }
   if (F == 0 || S == 0) return FASTFP_OK;
-  DeviceGuard g(pk->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  const bool fdev = flags & FASTFP_FREQS_ON_DEVICE, odev = flags & FASTFP_OUT_ON_DEVICE;
   const int P = pk->P;
-  const double* d_freqs = freqs;
-  if (!fdev) {
-    if (int rc = ensure(&pk->d_freqs, &pk->freqs_cap, F)) return rc;
-    FFP_CUDA(cudaMemcpyAsync(pk->d_freqs, freqs, (size_t)F * 8, cudaMemcpyHostToDevice, st));
-    d_freqs = pk->d_freqs;
-  }
-  double* d_out = out;
-  if (!odev) {
-    if (int rc = ensure(&pk->d_out, &pk->out_cap, S * F)) return rc;
-    d_out = pk->d_out;
-  }
+  PackCall c(pk, stream);
+  const double* d_freqs;
+  double* d_out;
+  if (int rc = c.stage(freqs, F, out, S * F, flags, &d_freqs, &d_out, &pk->d_out, &pk->out_cap)) return rc;
   const int64_t FB = std::max<int64_t>(1024, std::min<int64_t>(F, kTermBudgetDoubles / (5 * (int64_t)P)));
   // scratch: the inner products of one frequency batch, then the antenna patterns of the S sky positions
   if (int rc = ensure(&pk->d_inner, &pk->inner_cap, 5 * (int64_t)P * std::min(FB, F) + 2 * S * P)) return rc;
   double* d_fp = pk->d_inner + 5 * (int64_t)P * std::min(FB, F);
   double* d_fx = d_fp + S * P;
-  FFP_CUDA(cudaMemcpyAsync(d_fp, fplus, (size_t)S * P * 8, cudaMemcpyHostToDevice, st));
-  FFP_CUDA(cudaMemcpyAsync(d_fx, fcross, (size_t)S * P * 8, cudaMemcpyHostToDevice, st));
+  FFP_CUDA(cudaMemcpyAsync(d_fp, fplus, (size_t)S * P * 8, cudaMemcpyHostToDevice, c.st));
+  FFP_CUDA(cudaMemcpyAsync(d_fx, fcross, (size_t)S * P * 8, cudaMemcpyHostToDevice, c.st));
   for (int64_t lo = 0; lo < F; lo += FB) {
     const int64_t fb = std::min(FB, F - lo);
-    if (int rc = sweep_terms(pk, d_freqs + lo, fb, nullptr, st, pk->d_inner)) return rc;
-    if (int rc = launch_fe_combine(pk->d_inner, P, fb, d_fp, d_fx, S, d_out + lo, F, st)) return rc;
+    if (int rc = launch_sweep(pk, d_freqs + lo, fb, nullptr, c.st, nullptr, pk->d_inner)) return rc;
+    if (int rc = launch_fe_combine(pk->d_inner, P, fb, d_fp, d_fx, S, d_out + lo, F, c.st)) return rc;
   }
-  if (!odev) {
-    FFP_CUDA(cudaMemcpyAsync(out, d_out, (size_t)S * F * 8, cudaMemcpyDeviceToHost, st));
-    FFP_CUDA(cudaStreamSynchronize(st));
+  if (!(flags & FASTFP_OUT_ON_DEVICE)) {
+    FFP_CUDA(cudaMemcpyAsync(out, d_out, (size_t)S * F * 8, cudaMemcpyDeviceToHost, c.st));
+    FFP_CUDA(cudaStreamSynchronize(c.st));
   } else {
-    FFP_CUDA(cudaStreamSynchronize(st));  // fplus / fcross were read from caller-owned host memory
+    FFP_CUDA(cudaStreamSynchronize(c.st));  // fplus / fcross were read from caller-owned host memory
   }
   return FASTFP_OK;
 }
@@ -496,36 +468,25 @@ int fastfp_nmfp_sweep(const fastfp_pack_t* pk, const double* freqs, int64_t F,
   }
   if (!pk->nmfp) { set_error("this pack was built for plain Fp; use fastfp_fp_sweep"); return FASTFP_ERR_INVALID; }
   if (F == 0 || D == 0) return FASTFP_OK;
-  DeviceGuard g(pk->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  const bool fdev = flags & FASTFP_FREQS_ON_DEVICE, odev = flags & FASTFP_OUT_ON_DEVICE,
-             pdev = flags & FASTFP_PARAMS_ON_DEVICE;
-  const double* d_freqs = freqs;
-  if (!fdev) {
-    if (int rc = ensure(&pk->d_freqs, &pk->freqs_cap, F)) return rc;
-    FFP_CUDA(cudaMemcpyAsync(pk->d_freqs, freqs, (size_t)F * 8, cudaMemcpyHostToDevice, st));
-    d_freqs = pk->d_freqs;
-  }
+  PackCall c(pk, stream);
+  const double* d_freqs;
+  double* d_out;
+  if (int rc = c.stage(freqs, F, out, D * F, flags, &d_freqs, &d_out, &pk->d_out, &pk->out_cap)) return rc;
   const double* d_phi = phiinv_var;
-  double* d_phi_tmp = nullptr;
-  if (!pdev) {
-    FFP_CUDA(cudaMalloc(&d_phi_tmp, (size_t)D * pk->mvar_total * 8));
-    FFP_CUDA(cudaMemcpyAsync(d_phi_tmp, phiinv_var, (size_t)D * pk->mvar_total * 8,
-                             cudaMemcpyHostToDevice, st));
-    d_phi = d_phi_tmp;
+  DeviceBuf<double> d_phi_tmp;
+  if (!(flags & FASTFP_PARAMS_ON_DEVICE)) {
+    FFP_CUDA(dev_alloc(&d_phi_tmp, (size_t)D * pk->mvar_total));
+    FFP_CUDA(cudaMemcpyAsync(d_phi_tmp.get(), phiinv_var, (size_t)D * pk->mvar_total * 8,
+                             cudaMemcpyHostToDevice, c.st));
+    d_phi = d_phi_tmp.get();
   }
-  double* d_out = out;
-  if (!odev) {
-    if (int rc = ensure(&pk->d_out, &pk->out_cap, D * F)) { cudaFree(d_phi_tmp); return rc; }
-    d_out = pk->d_out;
-  }
-  int rc = nmfp_sweep_impl(pk, d_freqs, F, d_phi, D, d_out, st);
-  if (!rc && !odev) {
-    cudaError_t e = cudaMemcpyAsync(out, d_out, (size_t)D * F * 8, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  int rc = nmfp_sweep_impl(pk, d_freqs, F, d_phi, D, d_out, c.st);
+  if (!rc && !(flags & FASTFP_OUT_ON_DEVICE)) {
+    cudaError_t e = cudaMemcpyAsync(out, d_out, (size_t)D * F * 8, cudaMemcpyDeviceToHost, c.st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c.st);
     if (e != cudaSuccess) rc = cuda_fail(e, "copy nmfp result to host");
   }
-  if (d_phi_tmp) { cudaStreamSynchronize(st); cudaFree(d_phi_tmp); }
+  if (d_phi_tmp) cudaStreamSynchronize(c.st);  // the sweep reads the staged parameters until it ends
   return rc;
 }
 
@@ -542,8 +503,9 @@ int fastfp_nmfp_stage_a(const fastfp_pack_t* pk, const double* freqs_dev, int64_
     set_error("fastfp_nmfp_stage_a: not an nmfp pack, null argument or F <= 0");
     return FASTFP_ERR_INVALID;
   }
-  DeviceGuard g(pk->device);
-  return nmfp_stage_a_impl(pk, freqs_dev, F, z_dev, a_dev, (cudaStream_t)stream);
+  PackCall c(pk, stream);
+  if (int rc = c.select()) return rc;
+  return nmfp_stage_a_impl(pk, freqs_dev, F, z_dev, a_dev, c.st);
 }
 
 int fastfp_nmfp_stage_b(const fastfp_pack_t* pk, const double* freqs_dev, int64_t F, const double* z_dev,
@@ -555,9 +517,9 @@ int fastfp_nmfp_stage_b(const fastfp_pack_t* pk, const double* freqs_dev, int64_
     return FASTFP_ERR_INVALID;
   }
   if (D == 0) return FASTFP_OK;
-  DeviceGuard g(pk->device);
-  return nmfp_stage_b_only(pk, freqs_dev, F, z_dev, a_dev, (int)tiles_per_block, phiinv_var_dev, D, out_dev,
-                           (cudaStream_t)stream);
+  PackCall c(pk, stream);
+  if (int rc = c.select()) return rc;
+  return nmfp_stage_b_only(pk, freqs_dev, F, z_dev, a_dev, (int)tiles_per_block, phiinv_var_dev, D, out_dev, c.st);
 }
 
 int fastfp_nmfp_stage_timing(fastfp_pack_t* pk, int enable) {
@@ -582,9 +544,10 @@ int fastfp_powerlaw_phiinv(const fastfp_pack_t* pk, const double* const* Ffreqs,
     return FASTFP_ERR_INVALID;
   }
   if (D == 0) return FASTFP_OK;
-  DeviceGuard g(pk->device);
+  PackCall c(pk, stream);
+  if (int rc = c.select()) return rc;
   return powerlaw_phiinv_impl(pk, Ffreqs, log10_A, gamma, D, curn_Ffreqs, ncurn, curn_log10_A,
-                              curn_gamma, phiinv_var_dev, (cudaStream_t)stream);
+                              curn_gamma, phiinv_var_dev, c.st);
 }
 
 static int xcy_run(int device, int64_t n, int64_t m, const double* Nvec, const double* T, const double* sigma,
@@ -597,9 +560,9 @@ static int xcy_run(int device, int64_t n, int64_t m, const double* Nvec, const d
   if (!g.ok) { set_error("cannot select CUDA device " + std::to_string(device)); return FASTFP_ERR_CUDA; }
   cudaStream_t st = (cudaStream_t)stream;
   const size_t tot = (size_t)(4 * n + n * m + m * m) + (size_t)(m * m + 3 * m + 2);
-  double* d = nullptr;
-  FFP_CUDA(cudaMalloc(&d, tot * 8));
-  double *dN = d, *dx = dN + n, *dy = dx + n, *dx0 = dy + n, *dT = dx0 + n, *dS = dT + n * m, *dW = dS + m * m;
+  DeviceBuf<double> d;
+  FFP_CUDA(dev_alloc(&d, tot));
+  double *dN = d.get(), *dx = dN + n, *dy = dx + n, *dx0 = dy + n, *dT = dx0 + n, *dS = dT + n * m, *dW = dS + m * m;
   double* dO = dW + (m * m + 3 * m);
   cudaError_t e = cudaMemcpyAsync(dN, Nvec, n * 8, cudaMemcpyHostToDevice, st);
   if (e == cudaSuccess) e = cudaMemcpyAsync(dx, x, n * 8, cudaMemcpyHostToDevice, st);
@@ -615,7 +578,6 @@ static int xcy_run(int device, int64_t n, int64_t m, const double* Nvec, const d
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) rc = cuda_fail(e, "fastfp_xcy download");
   }
-  cudaFree(d);
   return rc;
 }
 
@@ -642,9 +604,9 @@ int fastfp_tnt(int device, int64_t n, int64_t m, const double* Nvec, const doubl
   cudaStream_t st = (cudaStream_t)stream;
   const int nsplit = (int)std::max<int64_t>(1, std::min<int64_t>(64, n / 256));
   const size_t tot = (size_t)(n + n * m + m + m * m) + (size_t)nsplit * m * m;
-  double* d = nullptr;
-  FFP_CUDA(cudaMalloc(&d, tot * 8));
-  double *dN = d, *dT = dN + n, *dP = dT + n * m, *dO = dP + m, *dW = dO + m * m;
+  DeviceBuf<double> d;
+  FFP_CUDA(dev_alloc(&d, tot));
+  double *dN = d.get(), *dT = dN + n, *dP = dT + n * m, *dO = dP + m, *dW = dO + m * m;
   cudaError_t e = cudaMemcpyAsync(dN, Nvec, n * 8, cudaMemcpyHostToDevice, st);
   if (e == cudaSuccess) e = cudaMemcpyAsync(dT, T, n * m * 8, cudaMemcpyHostToDevice, st);
   if (e == cudaSuccess && phiinv) e = cudaMemcpyAsync(dP, phiinv, m * 8, cudaMemcpyHostToDevice, st);
@@ -657,7 +619,6 @@ int fastfp_tnt(int device, int64_t n, int64_t m, const double* Nvec, const doubl
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) rc = cuda_fail(e, "fastfp_tnt download");
   }
-  cudaFree(d);
   return rc;
 }
 

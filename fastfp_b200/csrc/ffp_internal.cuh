@@ -5,6 +5,7 @@
 #include <stdint.h>
 
 #include <atomic>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -203,6 +204,20 @@ inline int ensure(T** buf, int64_t* cap, int64_t need) {
   FFP_CUDA(cudaMalloc(buf, (size_t)need * sizeof(T)));
   *cap = need;
   return 0;
+}
+
+// device memory a host function holds for one call: cudaFree'd when the holder goes out of scope, on every return path
+struct CudaFree {
+  void operator()(void* p) const { cudaFree(p); }
+};
+template <typename T>
+using DeviceBuf = std::unique_ptr<T, CudaFree>;
+template <typename T>
+inline cudaError_t dev_alloc(DeviceBuf<T>* buf, size_t count) {
+  T* p = nullptr;
+  const cudaError_t e = cudaMalloc(&p, count * sizeof(T));
+  buf->reset(e == cudaSuccess ? p : nullptr);
+  return e;
 }
 
 // ---- kernel launchers (defined in the .cu files) ---------------------------------------

@@ -758,19 +758,18 @@ int build_i8_planes(fastfp_pack* pk, cudaStream_t st) {
   FFP_CUDA(cudaMalloc(&pk->d_i8, (size_t)off + 16));
   FFP_CUDA(cudaMalloc(&pk->d_i8_scale, (size_t)P * i8::RS * sizeof(double)));
   FFP_CUDA(cudaMemsetAsync(pk->d_i8_scale, 0, (size_t)P * i8::RS * sizeof(double), st));
-  int *d_exp = nullptr, *d_bad = nullptr;
-  FFP_CUDA(cudaMalloc(&d_exp, (size_t)P * i8::RS * sizeof(int)));
-  FFP_CUDA(cudaMalloc(&d_bad, (size_t)P * sizeof(int)));
-  FFP_CUDA(cudaMemsetAsync(d_bad, 0, (size_t)P * sizeof(int), st));
-  i8::i8_rowscale_kernel<<<dim3(rows_max, P), 256, 0, st>>>(pk->d_packets, pk->d_meta, pk->d_i8_scale, d_exp, d_bad);
-  i8::i8_planes_kernel<<<dim3(nst_max, P), 256, 0, st>>>(pk->d_packets, pk->d_meta, d_exp, pk->d_i8);
+  DeviceBuf<int> d_exp, d_bad;
+  FFP_CUDA(dev_alloc(&d_exp, (size_t)P * i8::RS));
+  FFP_CUDA(dev_alloc(&d_bad, (size_t)P));
+  FFP_CUDA(cudaMemsetAsync(d_bad.get(), 0, (size_t)P * sizeof(int), st));
+  i8::i8_rowscale_kernel<<<dim3(rows_max, P), 256, 0, st>>>(pk->d_packets, pk->d_meta, pk->d_i8_scale, d_exp.get(),
+                                                            d_bad.get());
+  i8::i8_planes_kernel<<<dim3(nst_max, P), 256, 0, st>>>(pk->d_packets, pk->d_meta, d_exp.get(), pk->d_i8);
   g_launches += 2;
   cudaError_t e = cudaGetLastError();
   std::vector<int> bad(P, 0);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(bad.data(), d_bad, (size_t)P * sizeof(int), cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(bad.data(), d_bad.get(), (size_t)P * sizeof(int), cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  cudaFree(d_exp);
-  cudaFree(d_bad);
   if (e != cudaSuccess) return cuda_fail(e, "build_i8_planes");
   // pulsars with a non-finite G or w (singular Sigma, NaN data) cannot be carried by integer planes: fp64 kernel
   std::vector<int> take, rest_flag(P, 1);

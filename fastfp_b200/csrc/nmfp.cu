@@ -87,23 +87,22 @@ int nmfp_pack_finish(fastfp_pack* pk, const double* d_toas, const double* d_res,
   pk->mvpad = 8 * nmbv;
   nmfp_init_sigma_kernel<<<P, 256, 0, st>>>(pk->d_L, pk->d_meta, d_TNT, d_phiinv_fix);
   g_launches += 1;
-  double* d_ur = nullptr;
-  FFP_CUDA(cudaMalloc(&d_ur, (size_t)P * MAX_M * sizeof(double)));
-  int rc = launch_fp_precompute(pk, d_toas, d_res, d_Nvec, d_T, st, d_ur, bn);
+  DeviceBuf<double> d_ur;
+  FFP_CUDA(dev_alloc(&d_ur, (size_t)P * MAX_M));
+  int rc = launch_fp_precompute(pk, d_toas, d_res, d_Nvec, d_T, st, d_ur.get(), bn);
   if (!rc) {
     cudaError_t e = cudaMalloc(&pk->d_S0, (size_t)P * pk->mvpad * pk->mvpad * 8);
     if (e == cudaSuccess) e = cudaMalloc(&pk->d_zr, (size_t)P * pk->mvpad * 8);
     if (e != cudaSuccess) rc = cuda_fail(e, "nmfp pack allocation");
   }
   if (!rc) {
-    nmfp_extract_kernel<<<P, 256, 0, st>>>(pk->d_L, pk->d_meta, d_ur, pk->d_S0, pk->d_zr, pk->mvpad);
+    nmfp_extract_kernel<<<P, 256, 0, st>>>(pk->d_L, pk->d_meta, d_ur.get(), pk->d_S0, pk->d_zr, pk->mvpad);
     g_launches += 1;
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) rc = cuda_fail(e, "nmfp_extract_kernel");
     pk->bytes += (int64_t)P * pk->mvpad * (pk->mvpad + 1) * 8;
   }
-  cudaFree(d_ur);
   if (!rc) rc = build_i8_planes(pk, st);  // stage A on the tensor path when every pulsar fits its tile
   return rc;
 }

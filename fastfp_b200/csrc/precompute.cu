@@ -146,8 +146,12 @@ int launch_fp_precompute(fastfp_pack* pk, const double* d_toas, const double* d_
   const int P = pk->P;
   int nmax = 0;
   for (auto& m : pk->meta) nmax = m.nch * m.ci > nmax ? m.nch * m.ci : nmax;
+  DeviceBuf<double> ur_tmp;
   double* d_ur = d_ur_keep;
-  if (!d_ur) FFP_CUDA(cudaMalloc(&d_ur, (size_t)P * MAX_M * sizeof(double)));
+  if (!d_ur) {
+    FFP_CUDA(dev_alloc(&ur_tmp, (size_t)P * MAX_M));
+    d_ur = ur_tmp.get();
+  }
   chol_kernel<<<P, 256, 0, st>>>(pk->d_L, pk->d_meta, pk->d_info);
   dim3 g1((nmax + 127) / 128, P);
   build_packets_kernel<<<g1, 128, 0, st>>>(pk->d_packets, pk->d_meta, pk->d_L, d_toas, d_Nvec, d_T,
@@ -163,7 +167,6 @@ int launch_fp_precompute(fastfp_pack* pk, const double* d_toas, const double* d_
   // caller can ask which pulsar it was (fastfp_pack_factor_info; the Python mirror warns)
   pk->info.assign(P, 0);
   FFP_CUDA(cudaMemcpy(pk->info.data(), pk->d_info, sizeof(int) * P, cudaMemcpyDeviceToHost));
-  if (!d_ur_keep) FFP_CUDA(cudaFree(d_ur));
   return 0;
 }
 

@@ -17,6 +17,8 @@ No validation beyond shapes is added: NaN/Inf propagate silently exactly as in t
 """
 from __future__ import annotations
 
+import os
+
 import numpy as np
 
 from . import _cabi
@@ -72,11 +74,22 @@ class _PackCache:
     hashes every byte of the lists. To keep that off the critical path the sweep is started on the cached pack
     right away while the hash runs on a worker thread (or, for asynchronous device-resident calls, on this thread
     after the launch); if the hash shows the inputs changed, the pack is rebuilt and the sweep repeated -- the
-    caller never sees a result computed from stale data."""
+    caller never sees a result computed from stale data.
+
+    It also holds what the front ends share: the pulsars' TOAs and residuals, the device (default ``LOCAL_RANK``
+    or 0) and the sweep path (default ``FASTFP_B200_PATH`` or "auto"), resolved at construction."""
 
     _pack = None
     _pack_key = None
     _pack_shape = None
+
+    def __init__(self, psrs, device=None, path=None):
+        self.toas = [np.asarray(psr.toas, dtype=np.float64) for psr in psrs]
+        self.residuals = [np.asarray(psr.residuals, dtype=np.float64) for psr in psrs]
+        self.device = int(os.environ.get("LOCAL_RANK", "0")) if device is None else int(device)
+        self.path = path if path is not None else os.environ.get("FASTFP_B200_PATH", "auto")
+        if self.path not in ("auto", "fp64", "i8", "prefer-i8"):
+            raise ValueError("path must be 'auto', 'fp64', 'i8' or 'prefer-i8'")
 
     def invalidate(self):
         """Drop the cached device pack (the next call rebuilds it)."""
@@ -86,6 +99,30 @@ class _PackCache:
 
     def _build_pack(self, lists):  # -> _cabi.Pack
         raise NotImplementedError
+
+    def _create_pack(self, Nvecs, Ts, mats, m_fix=None, phiinv_fix=None):
+        """``_cabi.Pack.create`` on this object's pulsars and device, set to its sweep path."""
+        pack = _cabi.Pack.create(self.toas, self.residuals, Nvecs, Ts, mats, m_fix, phiinv_fix, device=self.device)
+        if self.path == "prefer-i8":  # the tensor kernel where the pack can take it, silently the fp64 one otherwise
+            for p in ("i8", "mixed"):
+                try:
+                    pack.set_path(p)
+                    break
+                except _cabi.FastFpError:
+                    pass
+        elif self.path != "auto":
+            pack.set_path(self.path)
+        return pack
+
+    def _device_freqs(self, fgw):
+        """A CUDA-tensor ``fgw`` as a flat contiguous tensor on the pack's device, and torch's current stream there."""
+        import torch
+
+        if fgw.dtype != torch.float64:
+            raise TypeError("fgw tensor must be float64 (the reference enables jax x64)")
+        if fgw.device.index != self.device:
+            raise ValueError(f"fgw is on {fgw.device}, the pack on cuda:{self.device}")
+        return fgw.contiguous().reshape(-1), torch.cuda.current_stream(fgw.device).cuda_stream
 
     def _ensure(self, lists, force=False, key=None):
         key = _fingerprint(lists) if key is None else key
@@ -136,38 +173,11 @@ class FastFp(_PackCache):
     def __init__(self, psrs, pta=None, device=None, path=None):
         self.psrs = psrs
         self.pta = pta
-        self.toas = [np.asarray(psr.toas, dtype=np.float64) for psr in psrs]
-        self.residuals = [np.asarray(psr.residuals, dtype=np.float64) for psr in psrs]
-        if device is None:
-            import os
-
-            device = int(os.environ.get("LOCAL_RANK", "0"))
-        self.device = int(device)
-        import os as _os
-
-        self.path = path if path is not None else _os.environ.get("FASTFP_B200_PATH", "auto")
-        if self.path not in ("auto", "fp64", "i8", "prefer-i8"):
-            raise ValueError("path must be 'auto', 'fp64', 'i8' or 'prefer-i8'")
+        super().__init__(psrs, device, path)
 
     # -- packing (one-time, frequency-independent precompute on the device) -----------------
     def _build_pack(self, lists):
-        from . import blockn
-
-        Nvecs, Ts, sigmas = lists
-        if any(blockn.is_block(N) for N in Nvecs):  # block-diagonal N (kernel ECORR)
-            pack = _cabi.Pack.create_blockn(self.toas, self.residuals, Nvecs, Ts, sigmas, device=self.device)
-        else:
-            pack = _cabi.Pack.create_fp(self.toas, self.residuals, Nvecs, Ts, sigmas, device=self.device)
-        if self.path == "prefer-i8":  # the tensor kernel where the pack can take it, silently the fp64 one otherwise
-            for p in ("i8", "mixed"):
-                try:
-                    pack.set_path(p)
-                    break
-                except _cabi.FastFpError:
-                    pass
-        elif self.path != "auto":
-            pack.set_path(self.path)
-        return pack
+        return self._create_pack(*lists)
 
     def prepare(self, Nvecs, Ts, sigmas, force=False):
         """Upload and pre-reduce the per-pulsar arrays. The pack is cached and keyed on the full contents
@@ -186,13 +196,8 @@ class FastFp(_PackCache):
         if _is_cuda_tensor(fgw):
             import torch
 
-            if fgw.dtype != torch.float64:
-                raise TypeError("fgw tensor must be float64 (the reference enables jax x64)")
-            if fgw.device.index != self.device:
-                raise ValueError(f"fgw is on {fgw.device}, the pack on cuda:{self.device}")
-            f = fgw.contiguous().reshape(-1)
+            f, stream = self._device_freqs(fgw)
             out = torch.empty(f.shape[0], dtype=torch.float64, device=f.device)
-            stream = torch.cuda.current_stream(f.device).cuda_stream
 
             def run(pack):
                 pack.fp_sweep((f.data_ptr(), f.shape[0]), out=out.data_ptr(), stream=stream)

@@ -49,13 +49,8 @@ class FastFe(FastFp):
         if _is_cuda_tensor(fgw):
             import torch
 
-            if fgw.dtype != torch.float64:
-                raise TypeError("fgw tensor must be float64")
-            if fgw.device.index != self.device:
-                raise ValueError(f"fgw is on {fgw.device}, the pack on cuda:{self.device}")
-            f = fgw.contiguous().reshape(-1)
+            f, stream = self._device_freqs(fgw)
             out = torch.empty((fplus.shape[0], f.shape[0]), dtype=torch.float64, device=f.device)
-            stream = torch.cuda.current_stream(f.device).cuda_stream
 
             def run(pack):
                 pack.fe_sweep((f.data_ptr(), f.shape[0]), fplus, fcross, out=out.data_ptr(), stream=stream)

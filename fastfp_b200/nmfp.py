@@ -18,11 +18,8 @@ arrays (what ``map_params`` builds, ``examples/run_nmfp.py:174-186``). Both batc
 """
 from __future__ import annotations
 
-import os
-
 import numpy as np
 
-from . import _cabi
 from . import constants as const
 from .fastfp import _PackCache, _is_cuda_tensor
 
@@ -211,12 +208,7 @@ class NMFP(_PackCache):
     def __init__(self, psrs, rn_sigs, device=None, path=None):
         self.psrs = psrs
         self.rn_sigs = rn_sigs
-        self.toas = [np.asarray(psr.toas, dtype=np.float64) for psr in psrs]
-        self.residuals = [np.asarray(psr.residuals, dtype=np.float64) for psr in psrs]
-        self.device = int(os.environ.get("LOCAL_RANK", "0")) if device is None else int(device)
-        self.path = path if path is not None else os.environ.get("FASTFP_B200_PATH", "auto")
-        if self.path not in ("auto", "fp64", "i8", "prefer-i8"):
-            raise ValueError("path must be 'auto', 'fp64', 'i8' or 'prefer-i8'")
+        super().__init__(psrs, device, path)
 
     def __call__(self, fgw, samples, Nvecs, Ts, TNTs):
         return self.calculate_nmfp(fgw, samples, Nvecs, Ts, TNTs)
@@ -235,8 +227,6 @@ class NMFP(_PackCache):
         return self._ensure((Nvecs, Ts, TNTs), force=force)
 
     def _build_pack(self, lists):
-        from . import blockn
-
         Nvecs, Ts, TNTs = lists
         fixed = [sig.fixed_phi() for sig in self.rn_sigs]
         m_fix = [f.shape[0] for f in fixed]
@@ -246,22 +236,7 @@ class NMFP(_PackCache):
                     f"pulsar {p}: basis has {np.shape(T)[1]} columns but the RN_container describes "
                     f"{m_fix[p]} fixed + {sig.Ffreqs.shape[0]} red-noise entries"
                 )
-        if any(blockn.is_block(N) for N in Nvecs):  # block-diagonal N (kernel ECORR)
-            pack = _cabi.Pack.create_blockn(self.toas, self.residuals, Nvecs, Ts, TNTs, m_fix,
-                                            [1.0 / f for f in fixed], device=self.device)
-        else:
-            pack = _cabi.Pack.create_nmfp(self.toas, self.residuals, Nvecs, Ts, TNTs, m_fix,
-                                          [1.0 / f for f in fixed], device=self.device)
-        if self.path == "prefer-i8":  # the tensor kernel where the pack can take it, silently the fp64 one otherwise
-            for p in ("i8", "mixed"):
-                try:
-                    pack.set_path(p)
-                    break
-                except _cabi.FastFpError:
-                    pass
-        elif self.path != "auto":
-            pack.set_path(self.path)
-        return pack
+        return self._create_pack(Nvecs, Ts, TNTs, m_fix, [1.0 / f for f in fixed])
 
     def _curn_setup(self):
         flags = {bool(sig.add_curn) for sig in self.rn_sigs}
@@ -354,17 +329,13 @@ class NMFP(_PackCache):
         curn, A, G, cA, cG, D, batched = self._draw_arrays(samples)
 
         dev = torch.device("cuda", self.device)
-        stream = torch.cuda.current_stream(dev).cuda_stream
         on_dev = _is_cuda_tensor(fgw)
         if on_dev:
-            if fgw.dtype != torch.float64:
-                raise TypeError("fgw tensor must be float64")
-            if fgw.device.index != self.device:
-                raise ValueError(f"fgw is on {fgw.device}, the pack on cuda:{self.device}")
-            f = fgw.contiguous().reshape(-1)
+            f, stream = self._device_freqs(fgw)
             out = torch.empty((D, f.shape[0]), dtype=torch.float64, device=dev)
         else:
             f = np.asarray(fgw, dtype=np.float64)
+            stream = torch.cuda.current_stream(dev).cuda_stream
 
         def run(pack):
             phiinv = torch.empty((D, pack.mvar_total), dtype=torch.float64, device=dev)
