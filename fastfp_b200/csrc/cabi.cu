@@ -63,7 +63,9 @@ static int pack_layout(fastfp_pack* pk, int P, const int64_t* n, const int64_t* 
     const int m_rows = blockn ? ((int)m[p] + 7) / 8 * 8 + 8 : (int)m[p];
     if (m[p] > MAX_M || !sweep_config(m_rows, &kc)) {
       set_error("pulsar " + std::to_string(p) + ": basis width m=" + std::to_string(m[p]) +
-                " exceeds the supported maximum " + std::to_string(MAX_M));
+                (blockn ? " exceeds the block-N maximum " + std::to_string(MAX_M - 8) + " (the widest kernel has " +
+                              std::to_string(MAX_M) + " rows, 8 of them hold the epoch slots)"
+                        : " exceeds the supported maximum " + std::to_string(MAX_M)));
       return FASTFP_ERR_UNSUPPORTED;
     }
     PulsarMeta& pm = pk->meta[p];

@@ -165,7 +165,10 @@ int fastfp_powerlaw_phiinv(const fastfp_pack_t* pack, const double* const* Ffreq
  *   residuals_w[p] = (N^-1 r) * Nvec,  Ts[p] = (N^-1 T) * Nvec row-wise,  Nvecs[p] = diagonal part
  *   (inf on padding TOAs);  mats[p] = sigma_p (m_fix == NULL: plain Fp) or TNT_p (nmfp, with m_fix /
  *   phiinv_fix as in fastfp_nmfp_pack_create), both formed with the block N.
- * The resulting pack is used with fastfp_fp_sweep / fastfp_nmfp_sweep unchanged. */
+ * The resulting pack is used with fastfp_fp_sweep / fastfp_nmfp_sweep unchanged.
+ * The epoch slots take 8 rows of the G tile after the basis rows (roundup8(m) + 8 in all), so a block-N pulsar
+ * has m <= 632: fastfp_sweep_chunk_toas(m, 1) returns 0 above that and fastfp_pack_create_blockn returns
+ * FASTFP_ERR_UNSUPPORTED. */
 int fastfp_sweep_chunk_toas(int64_t m, int blockn);
 int fastfp_pack_create_blockn(int device, int P, const int64_t* n, const int64_t* m,
                               const double* const* toas, const double* const* residuals,
