@@ -36,6 +36,8 @@ SYMBOLS = {
     "fastfp_fp_terms": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p]),
     "fastfp_fe_sweep": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
                                   C.c_int, C.c_void_p]),
+    "fastfp_fe_skymax": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                   C.c_void_p, C.c_int, C.c_void_p]),
     "fastfp_nmfp_pack_create": (
         C.c_int,
         [C.c_int, C.c_int, c_int64_p, c_int64_p, c_double_pp, c_double_pp, c_double_pp, c_double_pp,
@@ -333,6 +335,28 @@ class Pack:
         check(load().fastfp_fe_sweep(self._h, _vp(freqs), F, _vp(fplus), _vp(fcross), S, _vp(out), flags,
                                      C.c_void_p(stream)))
         return ret
+
+    def fe_skymax(self, freqs, fplus, fcross, out=None, index_out=None, stream: int = 0):
+        """Loudest of ``S`` sky positions per frequency: ``fplus``, ``fcross`` host arrays ``(S, P)``. Returns / fills
+        ``(fe_max, sky_index)``, ``(F,)`` float64 and int64. ``freqs`` / ``out`` as in :meth:`fp_sweep`; ``index_out``
+        is a host int64 array when ``out`` is on the host, a device address when ``out`` is one."""
+        fplus, fcross = as_f64(fplus), as_f64(fcross)
+        if fplus.ndim != 2 or fplus.shape != fcross.shape or fplus.shape[1] != self.P:
+            raise ValueError("fplus and fcross must both have shape (n_sky, n_pulsars)")
+        S = fplus.shape[0]
+        freqs, out, F, ret, flags = self._stage(freqs, out)
+        iret = None
+        if flags & OUT_ON_DEVICE:
+            if index_out is None or isinstance(index_out, np.ndarray):
+                raise ValueError("out is a device address, so index_out must be one too")
+        elif index_out is None:
+            index_out = iret = np.empty(F, dtype=np.int64)
+        elif not (isinstance(index_out, np.ndarray) and index_out.dtype == np.int64 and index_out.shape == (F,)
+                  and index_out.flags.c_contiguous):
+            raise ValueError("index_out must be a contiguous int64 host array of shape (F,)")
+        check(load().fastfp_fe_skymax(self._h, _vp(freqs), F, _vp(fplus), _vp(fcross), S, _vp(out), _vp(index_out),
+                                      flags, C.c_void_p(stream)))
+        return ret, iret
 
     def nmfp_sweep(self, freqs, phiinv_var, D: int, out=None, stream: int = 0):
         freqs, out, F, ret, flags = self._stage(freqs, out, D)

@@ -462,6 +462,56 @@ int fastfp_fe_sweep(const fastfp_pack_t* pk, const double* freqs, int64_t F, con
   return FASTFP_OK;
 }
 
+// Sky-maximised Fe: the same sweep per frequency batch, then a combine that reduces over the sky as it goes
+int fastfp_fe_skymax(const fastfp_pack_t* pk, const double* freqs, int64_t F, const double* fplus, const double* fcross,
+                     int64_t S, double* fe_max, int64_t* sky_index, int flags, void* stream) {
+  if (!pk || F < 0 || S < 0 || (F > 0 && (!freqs || !fe_max || !sky_index || (S > 0 && (!fplus || !fcross))))) {
+    set_error("fastfp_fe_skymax: null argument or negative size");
+    return FASTFP_ERR_INVALID;
+  }
+  if (pk->nmfp) { set_error("fastfp_fe_skymax needs a plain-Fp pack (fastfp_pack_create)"); return FASTFP_ERR_INVALID; }
+  if (F == 0) return FASTFP_OK;
+  if (S == 0) { set_error("fastfp_fe_skymax needs at least one sky position"); return FASTFP_ERR_INVALID; }
+  const int P = pk->P;
+  PackCall c(pk, stream);
+  const double* d_freqs;
+  double* d_max;
+  if (int rc = c.stage(freqs, F, fe_max, F, flags, &d_freqs, &d_max, &pk->d_out, &pk->out_cap)) return rc;
+  const int64_t FB = std::max<int64_t>(1024, std::min<int64_t>(F, kTermBudgetDoubles / (5 * (int64_t)P)));
+  const int64_t fb0 = std::min(FB, F);
+  const FeSkyPlan plan = fe_skymax_plan(fb0, S, pk->num_sms);
+  // scratch, all in the pack's Fe buffer: the inner products of one frequency batch, the antenna patterns and the
+  // weights of the S sky positions, the per-chunk bests of a split sky, and the indices on their way to host memory
+  // (int64, 8 bytes per slot like the doubles). Like every scratch buffer of the pack it grows on demand and is kept
+  // until the pack is destroyed: 5 P F_batch + 7 S P doubles, plus F for host outputs and a small split scratch; about
+  // 750 MB after a call with S = 196 608 and P = 68. Allocating it per call instead costs a cudaMalloc / cudaFree pair per call, measured at up
+  // to several times the whole call at C2 sizes.
+  const int64_t n_inner = 5 * (int64_t)P * fb0, n_part = plan.nchunk > 1 ? plan.nchunk * fb0 : 0;
+  const int64_t n_idx = (flags & FASTFP_OUT_ON_DEVICE) ? 0 : F;
+  if (int rc = ensure(&pk->d_inner, &pk->inner_cap, n_inner + 7 * S * P + 2 * n_part + n_idx)) return rc;
+  double* d_fp = pk->d_inner + n_inner;
+  double* d_fx = d_fp + S * P;
+  double* d_w = d_fx + S * P;
+  double* part_v = d_w + 5 * S * P;
+  int64_t* part_i = reinterpret_cast<int64_t*>(part_v + n_part);
+  int64_t* d_idx = n_idx ? part_i + n_part : sky_index;
+  FFP_CUDA(cudaMemcpyAsync(d_fp, fplus, (size_t)S * P * 8, cudaMemcpyHostToDevice, c.st));
+  FFP_CUDA(cudaMemcpyAsync(d_fx, fcross, (size_t)S * P * 8, cudaMemcpyHostToDevice, c.st));
+  if (int rc = launch_fe_sky_weights(d_fp, d_fx, S * P, d_w, c.st)) return rc;
+  for (int64_t lo = 0; lo < F; lo += FB) {
+    const int64_t fb = std::min(FB, F - lo);
+    if (int rc = launch_sweep(pk, d_freqs + lo, fb, nullptr, c.st, nullptr, pk->d_inner)) return rc;
+    if (int rc = launch_fe_skymax(pk->d_inner, P, fb, d_w, S, plan, part_v, part_i, d_max + lo, d_idx + lo, c.st))
+      return rc;
+  }
+  if (!(flags & FASTFP_OUT_ON_DEVICE)) {
+    FFP_CUDA(cudaMemcpyAsync(fe_max, d_max, (size_t)F * 8, cudaMemcpyDeviceToHost, c.st));
+    FFP_CUDA(cudaMemcpyAsync(sky_index, d_idx, (size_t)F * 8, cudaMemcpyDeviceToHost, c.st));
+  }
+  FFP_CUDA(cudaStreamSynchronize(c.st));  // fplus / fcross were read from caller-owned host memory
+  return FASTFP_OK;
+}
+
 int fastfp_nmfp_sweep(const fastfp_pack_t* pk, const double* freqs, int64_t F,
                       const double* phiinv_var, int64_t D, double* out, int flags, void* stream) {
   if (!pk || F < 0 || D < 0 || ((F > 0 && D > 0) && (!freqs || !phiinv_var || !out))) {

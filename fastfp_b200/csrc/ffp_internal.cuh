@@ -252,6 +252,16 @@ int launch_fp_sweep_i8(const fastfp_pack* pk, const double* d_freqs, int64_t F, 
 // fe.cu
 int launch_fe_combine(const double* d_inner, int P, int64_t F, const double* d_fplus, const double* d_fcross, int64_t S,
                       double* d_out, int64_t out_ld, cudaStream_t st);
+// sky maximum: d_w = (S, P, 5) weights from launch_fe_sky_weights; a plan with nchunk > 1 needs the (nchunk, F)
+// scratch d_part_v / d_part_i for the per-chunk bests
+struct FeSkyPlan {
+  int64_t chunk;   // sky positions per chunk (a multiple of the pass width)
+  int64_t nchunk;  // chunks along the sky axis
+};
+FeSkyPlan fe_skymax_plan(int64_t F, int64_t S, int num_sms);
+int launch_fe_sky_weights(const double* d_fplus, const double* d_fcross, int64_t n, double* d_w, cudaStream_t st);
+int launch_fe_skymax(const double* d_inner, int P, int64_t F, const double* d_w, int64_t S, const FeSkyPlan& pl,
+                     double* d_part_v, int64_t* d_part_i, double* d_best, int64_t* d_idx, cudaStream_t st);
 bool sweep_config(int m, KernelCfg* cfg);
 int sweep_max_slab_doubles();
 // xcy.cu

@@ -68,3 +68,40 @@ class FastFe(FastFp):
         return np.float64(res) if np.ndim(res) == 0 else res
 
     compute_Fe = calculate_Fe
+
+    def calculate_Fe_skymax(self, fgw, gwtheta, gwphi, Nvecs, Ts, sigmas):
+        """The loudest position of the sky grid ``gwtheta``, ``gwphi`` (broadcast to ``(S,)``) at each frequency
+        ``fgw``, without forming the ``(S, F)`` map of :meth:`calculate_Fe` (``fastfp_fe_skymax``). Returns
+        ``(fe_max, sky_index)``: ``(float, int)`` for a scalar ``fgw``, ``float64`` and ``int64`` arrays of
+        ``fgw``'s shape for an array, CUDA tensors on its device (enqueued on torch's current stream) for a float64
+        CUDA tensor. Each value equals the corresponding entry of :meth:`calculate_Fe`'s map bit for bit; NaN loses,
+        ties go to the lowest index, and a frequency with no finite value gives ``(nan, -1)``."""
+        try:
+            th, ph = np.broadcast_arrays(np.atleast_1d(np.asarray(gwtheta, dtype=np.float64)),
+                                         np.atleast_1d(np.asarray(gwphi, dtype=np.float64)))
+        except ValueError:
+            raise ValueError("gwtheta and gwphi must broadcast to one shape (S,)") from None
+        if th.ndim != 1:
+            raise ValueError("gwtheta and gwphi must broadcast to one shape (S,)")
+        fplus, fcross = antenna_pattern(self.pos, th, ph)  # (S, P)
+        lists = (Nvecs, Ts, sigmas)
+        if _is_cuda_tensor(fgw):
+            import torch
+
+            f, stream = self._device_freqs(fgw)
+            best = torch.empty(f.shape[0], dtype=torch.float64, device=f.device)
+            idx = torch.empty(f.shape[0], dtype=torch.int64, device=f.device)
+
+            def run(pack):
+                pack.fe_skymax((f.data_ptr(), f.shape[0]), fplus, fcross, out=best.data_ptr(),
+                               index_out=idx.data_ptr(), stream=stream)
+                return best, idx
+
+            best, idx = self._run_verified(lists, run, asynchronous=True)
+            return best.reshape(fgw.shape), idx.reshape(fgw.shape)
+        f = np.asarray(fgw, dtype=np.float64)
+        best, idx = self._run_verified(lists, lambda pack: pack.fe_skymax(f.reshape(-1), fplus, fcross),
+                                       asynchronous=False)
+        if f.ndim == 0:
+            return float(best[0]), int(idx[0])
+        return best.reshape(f.shape), idx.reshape(f.shape)

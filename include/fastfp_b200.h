@@ -105,6 +105,21 @@ int fastfp_fp_terms(const fastfp_pack_t* pack, const double* freqs, int64_t F, d
 int fastfp_fe_sweep(const fastfp_pack_t* pack, const double* freqs, int64_t F, const double* fplus,
                     const double* fcross, int64_t S, double* out, int flags, void* stream);
 
+/* fastfp_fe_skymax: the loudest sky position per frequency of an all-sky scan, without the (S, F) map:
+ *   fe_max[f] = max_s Fe(s, f),   sky_index[f] = the s that attains it           (fe_max, sky_index: (F,) each)
+ * Every Fe(s, f) is the value fastfp_fe_sweep returns for it, bit for bit. Reduction rule: a NaN loses to every other
+ * value; among equal values the lowest sky index wins; a frequency where every position is NaN (e.g. f <= 0) gives
+ * fe_max = NaN and sky_index = -1. The result does not depend on how the work is split. fplus, fcross: host arrays
+ * (S, P) row-major as for fastfp_fe_sweep; S is limited by device memory only (scratch below).
+ * flags as for fastfp_fp_sweep; FASTFP_OUT_ON_DEVICE covers both outputs. Returns FASTFP_ERR_INVALID for a NULL
+ * argument, a negative size, an nmfp pack, or S == 0 with F > 0; F == 0 returns FASTFP_OK and writes nothing.
+ * Device scratch: the call grows the pack's Fe scratch to 5 P F_batch + 7 S P doubles (one frequency batch of inner
+ * products, the antenna patterns and the per-(sky, pulsar) weights; about 750 MB for S = 196 608, P = 68, against
+ * 2 S P for the patterns of fastfp_fe_sweep), plus F for host outputs; the pack keeps it, like
+ * its other scratch buffers, until fastfp_pack_destroy, so repeated calls allocate nothing. */
+int fastfp_fe_skymax(const fastfp_pack_t* pack, const double* freqs, int64_t F, const double* fplus,
+                     const double* fcross, int64_t S, double* fe_max, int64_t* sky_index, int flags, void* stream);
+
 /* ---- noise-marginalised Fp -----------------------------------------------------------
  * fastfp_nmfp_pack_create: NMFP.__init__ (fastfp/nmfp.py:45-51) plus the (TNTs, Nvecs, Ts)
  * of get_mats_nmfp (fastfp/utils.py:97-101). Sigma_d = TNT + diag(phiinv_d) is formed per
