@@ -38,6 +38,8 @@ SYMBOLS = {
                                   C.c_int, C.c_void_p]),
     "fastfp_fe_skymax": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
                                    C.c_void_p, C.c_int, C.c_void_p]),
+    "fastfp_pack_set_residuals": (C.c_int, [C.c_void_p, C.c_int64, c_double_pp, C.c_void_p]),
+    "fastfp_fp_sweep_residuals": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p]),
     "fastfp_nmfp_pack_create": (
         C.c_int,
         [C.c_int, C.c_int, c_int64_p, c_int64_p, c_double_pp, c_double_pp, c_double_pp, c_double_pp,
@@ -93,6 +95,15 @@ SYMBOLS = {
     ),
     "fastfp_fp64_peak": (C.c_int, [C.c_int, C.c_int, C.c_int, c_double_p, c_double_p]),
 }
+
+
+MAX_M = 640  # G rows of the widest sweep kernel (csrc/ffp_internal.cuh)
+
+
+def max_residual_rows(m) -> int:
+    """Most residual realisations ``fastfp_pack_set_residuals`` takes for pulsars of basis widths ``m``: every pulsar
+    needs ``roundup8(m_p) + roundup8(R)`` of the sweep kernel's ``MAX_M`` G rows."""
+    return MAX_M - -(-max(m) // 8) * 8
 
 
 class FastFpError(RuntimeError):
@@ -207,6 +218,8 @@ class Pack:
         self._warn_if_not_spd()
 
     PATHS = {"auto": 0, "fp64": 1, "i8": 2, "mixed": 3}
+    blockn = False  # a block-diagonal N (set by create)
+    R = 0           # realisations set by set_residuals
 
     def set_path(self, path: str) -> None:
         """Kernel of the plain-Fp sweep: "auto" (default: the fp64 DMMA kernel), "fp64", "i8" (the INT8
@@ -294,7 +307,9 @@ class Pack:
             check(lib.fastfp_nmfp_pack_create(*head, *map(_ptr_array, (toas, residuals, Nvecs, Ts, mats)), *fixed, *tail))
         else:
             check(lib.fastfp_pack_create(*head, *map(_ptr_array, (toas, residuals, Nvecs, Ts, mats)), *tail))
-        return cls(h, P, device, nmfp, n, m)
+        pack = cls(h, P, device, nmfp, n, m)
+        pack.blockn = block
+        return pack
 
     # -- sweeps -------------------------------------------------------------------------
     @staticmethod
@@ -357,6 +372,30 @@ class Pack:
         check(load().fastfp_fe_skymax(self._h, _vp(freqs), F, _vp(fplus), _vp(fcross), S, _vp(out), _vp(index_out),
                                       flags, C.c_void_p(stream)))
         return ret, iret
+
+    def set_residuals(self, residuals, stream: int = 0) -> None:
+        """Realisations of the residuals for :meth:`fp_sweep_residuals`: ``residuals[p]`` is ``(R, n_p)`` (host); the
+        pack keeps them until the next call. ``R`` is at most :func:`max_residual_rows` of the pack's widths; an
+        empty list of rows (``R == 0``) releases them."""
+        if self.blockn:  # its TOAs are re-laid out by epoch (blockn.prepare); the library refuses these packs too
+            raise FastFpError("residual batches need a diagonal-N pack; this one has a block-diagonal N")
+        if len(residuals) != self.P:
+            raise ValueError(f"residuals must be a list of {self.P} arrays (one per pulsar)")
+        res = [as_f64(r) for r in residuals]
+        R = res[0].shape[0] if res[0].ndim == 2 else -1
+        for p, r in enumerate(res):
+            if r.shape != (R, self.n[p]):
+                raise ValueError(f"residuals[{p}] must have shape (R, {self.n[p]}) with the same R for every pulsar; "
+                                 f"got {r.shape}")
+        check(load().fastfp_pack_set_residuals(self._h, R, _ptr_array(res), C.c_void_p(stream)))
+        self.R = R
+
+    def fp_sweep_residuals(self, freqs, out=None, stream: int = 0):
+        """Fp of each realisation set by :meth:`set_residuals`: ``(R, F)``. ``freqs`` / ``out`` as in
+        :meth:`fp_sweep`. Always the fp64 kernel, whatever :attr:`path` says."""
+        freqs, out, F, ret, flags = self._stage(freqs, out, self.R)
+        check(load().fastfp_fp_sweep_residuals(self._h, _vp(freqs), F, _vp(out), flags, C.c_void_p(stream)))
+        return ret
 
     def nmfp_sweep(self, freqs, phiinv_var, D: int, out=None, stream: int = 0):
         freqs, out, F, ret, flags = self._stage(freqs, out, D)

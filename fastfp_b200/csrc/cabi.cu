@@ -174,6 +174,7 @@ static void pack_free(fastfp_pack* pk) {
   cudaFree(pk->d_pl); cudaFreeHost(pk->h_pl);
   cudaFree(pk->d_i8); cudaFree(pk->d_i8_scale); cudaFree(pk->d_pidx_all); cudaFree(pk->d_inner);
   if (pk->pl_event) cudaEventDestroy(pk->pl_event);
+  res_release(pk);
   delete pk;
 }
 
@@ -367,7 +368,7 @@ int fastfp_pack_create_blockn(int device, int P, const int64_t* n, const int64_t
 }
 
 void fastfp_pack_destroy(fastfp_pack_t* pack) { pack_free(pack); }
-int64_t fastfp_pack_bytes(const fastfp_pack_t* pack) { return pack ? pack->bytes : 0; }
+int64_t fastfp_pack_bytes(const fastfp_pack_t* pack) { return pack ? pack->bytes + pack->res_bytes : 0; }
 int fastfp_pack_num_pulsars(const fastfp_pack_t* pack) { return pack ? pack->P : 0; }
 int64_t fastfp_pack_mvar_total(const fastfp_pack_t* pack) { return pack ? pack->mvar_total : 0; }
 int fastfp_pack_factor_info(const fastfp_pack_t* pack, int32_t* info) {
@@ -425,6 +426,78 @@ int fastfp_fp_sweep(const fastfp_pack_t* pack, const double* freqs, int64_t F, d
 int fastfp_fp_terms(const fastfp_pack_t* pack, const double* freqs, int64_t F, double* terms,
                     int flags, void* stream) {
   return fp_run(pack, freqs, F, terms, flags, stream, true);
+}
+
+// Residual batches (DESIGN.md section 5d): R realisations of the residuals as extra G rows of the fp64 kernel
+int fastfp_pack_set_residuals(fastfp_pack_t* pk, int64_t R, const double* const* residuals, void* stream) {
+  if (!pk || R < 0 || (R > 0 && !residuals)) {
+    set_error("fastfp_pack_set_residuals: null argument or negative R");
+    return FASTFP_ERR_INVALID;
+  }
+  if (pk->nmfp) { set_error("fastfp_pack_set_residuals needs a plain-Fp pack (fastfp_pack_create)"); return FASTFP_ERR_INVALID; }
+  if (pk->ecorr) {
+    set_error("fastfp_pack_set_residuals: block-diagonal N packs are not supported");
+    return FASTFP_ERR_UNSUPPORTED;
+  }
+  int wide = 0;
+  for (int p = 0; p < pk->P; ++p) {
+    if (R > 0 && !residuals[p]) { set_error("fastfp_pack_set_residuals: null per-pulsar array"); return FASTFP_ERR_INVALID; }
+    if (pk->meta[p].m > pk->meta[wide].m) wide = p;
+  }
+  const int64_t rmax = MAX_M - (pk->meta[wide].m + 7) / 8 * 8;
+  if (R > rmax) {
+    set_error("fastfp_pack_set_residuals: R = " + std::to_string(R) + " exceeds the limit of " + std::to_string(rmax) +
+              " for this pack: its widest pulsar " + std::to_string(wide) + " (m = " + std::to_string(pk->meta[wide].m) +
+              ") leaves " + std::to_string(rmax) + " of the sweep kernel's " + std::to_string(MAX_M) + " G rows");
+    return FASTFP_ERR_UNSUPPORTED;
+  }
+  PackCall c(pk, stream);
+  if (int rc = c.select()) return rc;
+  FFP_CUDA(cudaStreamSynchronize(c.st));  // sweeps queued on this stream may still read the previous set
+  res_release(pk);
+  if (R == 0) return FASTFP_OK;
+  const int64_t n_tot = pk->meta.back().raw_off + pk->meta.back().n;
+  DeviceBuf<double> d_res;
+  FFP_CUDA(dev_alloc(&d_res, (size_t)(R * n_tot)));
+  for (int p = 0; p < pk->P; ++p) {
+    const PulsarMeta& pm = pk->meta[p];
+    FFP_CUDA(cudaMemcpyAsync(d_res.get() + R * pm.raw_off, residuals[p], (size_t)(R * pm.n) * 8,
+                             cudaMemcpyHostToDevice, c.st));
+  }
+  const int rc = build_res_packets(pk, R, d_res.get(), c.st);
+  if (rc) res_release(pk);
+  return rc;
+}
+
+int fastfp_fp_sweep_residuals(const fastfp_pack_t* pk, const double* freqs, int64_t F, double* out, int flags,
+                              void* stream) {
+  if (!pk || F < 0 || (F > 0 && (!freqs || !out))) {
+    set_error("fastfp_fp_sweep_residuals: null argument or negative F");
+    return FASTFP_ERR_INVALID;
+  }
+  if (pk->res_R == 0) {
+    set_error("fastfp_fp_sweep_residuals: no residual realisations set (fastfp_pack_set_residuals)");
+    return FASTFP_ERR_INVALID;
+  }
+  if (F == 0) return FASTFP_OK;
+  const int P = pk->P;
+  const int64_t R = pk->res_R;
+  PackCall c(pk, stream);
+  const double* d_freqs;
+  double* d_out;
+  if (int rc = c.stage(freqs, F, out, R * F, flags, &d_freqs, &d_out, &pk->d_out, &pk->out_cap)) return rc;
+  const int64_t FB = std::max<int64_t>(1024, std::min<int64_t>(F, kTermBudgetDoubles / (R * P)));
+  if (int rc = ensure(&pk->d_res_terms, &pk->res_terms_cap, R * P * std::min(FB, F))) return rc;
+  for (int64_t lo = 0; lo < F; lo += FB) {
+    const int64_t fb = std::min(FB, F - lo);
+    if (int rc = launch_fp_sweep_res(pk, d_freqs + lo, fb, pk->d_res_terms, c.st)) return rc;
+    if (int rc = launch_reduce_terms_rows(pk->d_res_terms, (int)R, P, fb, d_out + lo, F, c.st)) return rc;
+  }
+  if (!(flags & FASTFP_OUT_ON_DEVICE)) {
+    FFP_CUDA(cudaMemcpyAsync(out, d_out, (size_t)(R * F) * 8, cudaMemcpyDeviceToHost, c.st));
+    FFP_CUDA(cudaStreamSynchronize(c.st));
+  }
+  return FASTFP_OK;
 }
 
 // Fe-statistic sky scan: one sweep for the inner products of every (pulsar, frequency), then the combine kernel

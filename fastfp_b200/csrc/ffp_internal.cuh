@@ -177,6 +177,15 @@ struct fastfp_pack {
   mutable int64_t pl_cap = 0;
   mutable cudaEvent_t pl_event = nullptr;
   mutable std::vector<double> pl_tab;
+  // residual batch (fastfp_pack_set_residuals, DESIGN.md section 5d): per pulsar, the G rows followed by the res_R
+  // realisations' w_k rows from row roundup8(m) on, in packets of the kernel configuration for that many rows
+  int64_t res_R = 0;
+  int64_t res_bytes = 0;
+  double* d_res_packets = nullptr;
+  ffp::PulsarMeta* d_res_meta = nullptr;
+  std::vector<ffp::Group> res_groups;
+  mutable double* d_res_terms = nullptr;  // [R][P][F_batch] terms of one frequency batch
+  mutable int64_t res_terms_cap = 0;
   // optional per-stage timing of nmfp sweeps (fastfp_nmfp_stage_timing): stage A, factor, stage B
   mutable bool time_stages = false;
   mutable double stage_ms[3] = {0.0, 0.0, 0.0};
@@ -231,6 +240,10 @@ int launch_fp_precompute(fastfp_pack* pk, const double* d_toas, const double* d_
                          const double* d_Nvec, const double* d_T, cudaStream_t st,
                          double* d_ur_keep = nullptr,  // [P][MAX_M], receives G r
                          const BlockNDev* bn = nullptr);
+// the residual packets of R realisations (d_res: per pulsar (R, n_p) row-major at R * raw_off); replaces any earlier
+// set. res_release frees them (R = 0).
+int build_res_packets(fastfp_pack* pk, int64_t R, const double* d_res, cudaStream_t st);
+void res_release(fastfp_pack* pk);
 // fp_sweep*.cu
 struct NmfpOut {      // stage-A outputs of the nmfp path (null for plain Fp)
   double* Z;          // [P][ceil(F/32)][mvpad/4][8][32]  z'_s, z'_c tiles in MMA B-fragment order
@@ -243,6 +256,11 @@ int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, dou
 int launch_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, double* d_terms, cudaStream_t st,
                  const NmfpOut* nm = nullptr, double* d_inner = nullptr);
 int launch_reduce_terms(const double* d_terms, int P, int64_t F, double* d_out, cudaStream_t st);
+// residual batches: the sweep over the pack's residual packets (terms [R][P][F]) and the pulsar sum of each row
+// into out[k * ld + f]
+int launch_fp_sweep_res(const fastfp_pack* pk, const double* d_freqs, int64_t F, double* d_terms, cudaStream_t st);
+int launch_reduce_terms_rows(const double* d_terms, int R, int P, int64_t F, double* d_out, int64_t ld,
+                             cudaStream_t st);
 // fp_sweep_i8.cu
 bool i8_eligible(const fastfp_pack* pk);
 int build_i8_planes(fastfp_pack* pk, cudaStream_t st);

@@ -35,6 +35,15 @@ __global__ void reduce_terms_kernel(const double* __restrict__ terms, int P, int
   out[f] = acc;
 }
 
+static int dispatch_group(const fastfp_pack* pk, const Group& g, const SweepArgs& a, bool nmfp, bool res,
+                          cudaStream_t st) {
+  if (g.cfg.wmw == 8) return dispatch_sweep_xwide(pk, g, a, nmfp, res, st);
+  if (g.cfg.wmw == 4) return dispatch_sweep_wide(pk, g, a, nmfp, res, st);
+  if (g.cfg.wmw == 1 && g.cfg.nnb == 4) return dispatch_sweep_w1(pk, g, a, nmfp, res, st);
+  if (g.cfg.wmw == 1) return dispatch_sweep_w2(pk, g, a, nmfp, res, st);
+  return dispatch_sweep_w4(pk, g, a, nmfp, res, st);
+}
+
 int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, double* d_terms,
                     cudaStream_t st, const NmfpOut* nm, double* d_inner, bool rest_only) {
 #ifdef FFP_DEBUG_SWITCHES  // profiling builds only; the shipped library is compiled without it
@@ -63,13 +72,7 @@ int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, dou
       g.count = g0.count_rest;
       g.d_pidx = g0.d_pidx_rest;
     }
-    int rc;
-    if (g.cfg.wmw == 8) rc = dispatch_sweep_xwide(pk, g, a, nm != nullptr, st);
-    else if (g.cfg.wmw == 4) rc = dispatch_sweep_wide(pk, g, a, nm != nullptr, st);
-    else if (g.cfg.wmw == 1 && g.cfg.nnb == 4) rc = dispatch_sweep_w1(pk, g, a, nm != nullptr, st);
-    else if (g.cfg.wmw == 1) rc = dispatch_sweep_w2(pk, g, a, nm != nullptr, st);
-    else rc = dispatch_sweep_w4(pk, g, a, nm != nullptr, st);
-    if (rc) return rc;
+    if (int rc = dispatch_group(pk, g, a, nm != nullptr, false, st)) return rc;
   }
   return 0;
 }
@@ -79,6 +82,43 @@ int launch_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, double
   if (!pk->use_i8()) return launch_fp_sweep(pk, d_freqs, F, d_terms, st, nm, d_inner);
   if (int rc = launch_fp_sweep_i8(pk, d_freqs, F, d_terms, st, d_inner, nm)) return rc;
   return pk->i8_all() ? 0 : launch_fp_sweep(pk, d_freqs, F, d_terms, st, nm, d_inner, true);
+}
+
+// The residual batch (DESIGN.md section 5d): the fp64 kernel on the pack's residual packets, whose G tiles carry
+// the realisations' w_k as extra rows; terms is [R][P][F].
+int launch_fp_sweep_res(const fastfp_pack* pk, const double* d_freqs, int64_t F, double* d_terms, cudaStream_t st) {
+  SweepArgs a{};
+  a.packets = pk->d_res_packets;
+  a.meta = pk->d_res_meta;
+  a.freqs = d_freqs;
+  a.F = F;
+  a.terms = d_terms;
+  a.slab = pk->d_slab;
+  a.counter = pk->d_counter;
+  a.nres = (int)pk->res_R;
+  a.npsr = pk->P;
+  for (const Group& g : pk->res_groups)
+    if (int rc = dispatch_group(pk, g, a, false, true, st)) return rc;
+  return 0;
+}
+
+// out[k * ld + f] = sum over pulsars of terms[k][p][f], in pulsar order from 0 (as reduce_terms_kernel)
+__global__ void reduce_terms_rows_kernel(const double* __restrict__ terms, int P, int64_t F,
+                                         double* __restrict__ out, int64_t ld) {
+  const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= F) return;
+  const double* t = terms + (size_t)blockIdx.y * P * F;
+  double acc = 0.0;
+  for (int p = 0; p < P; ++p) acc += t[(size_t)p * F + f];
+  out[(size_t)blockIdx.y * ld + f] = acc;
+}
+
+int launch_reduce_terms_rows(const double* d_terms, int R, int P, int64_t F, double* d_out, int64_t ld,
+                             cudaStream_t st) {
+  reduce_terms_rows_kernel<<<dim3((unsigned)((F + 255) / 256), (unsigned)R), 256, 0, st>>>(d_terms, P, F, d_out, ld);
+  g_launches += 1;
+  FFP_CUDA(cudaGetLastError());
+  return 0;
 }
 
 int launch_reduce_terms(const double* d_terms, int P, int64_t F, double* d_out, cudaStream_t st) {

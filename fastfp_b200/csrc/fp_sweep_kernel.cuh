@@ -54,6 +54,8 @@ struct SweepArgs {
   double* A;              // nmfp: [P][ceil(F/32)][5][32]
   int mvmax;
   const unsigned char* done_mask;  // block-N packs: per chunk, which of the 8 epoch slots end there
+  int nres;   // residual batches: realisations, in rows roundup8(m) .. roundup8(m)+nres-1 of G; terms is [nres][npsr][F]
+  int npsr;
 #ifdef FFP_DEBUG_SWITCHES
   int dbg;  // profiling builds only (tools/dbg_split.sh): bit 0 producers' math off, 1 MMAs off, 2 level-2 flush off
 #endif
@@ -259,7 +261,9 @@ __device__ __forceinline__ void producer_loop(const SweepArgs& ar, SweepSmem<C>&
 }
 
 // ---- consumer role: the contraction and the epilogue -----------------------------------------
-template <class C, bool NMFP, bool ECORR>
+// RES: residual batches (DESIGN.md section 5d). Rows from roundup8(m) on hold w_k = C^-1 r_k, so Y there is
+// ((s|r_k), (c|r_k)); the epilogue solves one 2x2 system per (realisation, frequency) with the shared M.
+template <class C, bool NMFP, bool ECORR, bool RES>
 __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>& sm, volatile int* s_work,
                                               const int cw, const int lane) {
   constexpr int NMBW = C::NMBW, NNB = C::NNB;
@@ -498,6 +502,11 @@ __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>&
         o[64] = a[2] - b[2];
         o[96] = a[3];
         o[128] = a[4];
+      } else if (RES) {
+        // M of this frequency for every realisation; slot 0 of redB for this frequency is read by this thread only
+        redB[tid * 3 + 0] = a[0] - b[0];
+        redB[tid * 3 + 1] = a[1] - b[1];
+        redB[tid * 3 + 2] = a[2] - b[2];
       } else {
         // M = [[ss, sc],[sc, cc]], N = [(s|r), (c|r)]
         double val = term_2x2(a[0] - b[0], a[1] - b[1], a[2] - b[2], a[3], a[4]);
@@ -509,11 +518,31 @@ __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>&
         }
       }
     }
+    if (RES) {
+      asm volatile("bar.sync 1, %0;" ::"n"(C::NTC) : "memory");  // consumers only: M of every frequency is published
+      const int r0 = (pm.m + 7) & ~7;
+#pragma unroll
+      for (int q = 0; q < NNB; ++q) {
+        const int fl = 4 * (wn * NNB + q) + (lane & 3);
+        const int64_t f = f0 + fl;
+        if (f >= ar.F) continue;
+        const double m00 = redB[fl * 3], m01 = redB[fl * 3 + 1], m11 = redB[fl * 3 + 2];
+        const bool fpos = sm.fq[fl] > 0.0;
+#pragma unroll
+        for (int r = 0; r < NMBW; ++r) {
+          const int k = 8 * (wm * NMBW + r) + (lane >> 2) - r0;
+          if (k < 0 || k >= ar.nres) continue;
+          double val = term_2x2(m00, m01, m11, acc[r][q][0], acc[r][q][1]);
+          if (!fpos) val = __longlong_as_double(0x7ff8000000000000LL);
+          ar.terms[((size_t)k * ar.npsr + p) * ar.F + f] = val;
+        }
+      }
+    }
     __syncthreads();  // B4: fq, red and s_work are reused by the next work item
   }
 }
 
-template <class C, bool NMFP, bool ECORR>
+template <class C, bool NMFP, bool ECORR, bool RES>
 __global__ void __launch_bounds__(C::NTHREADS, CTAS_PER_SM) fp_sweep_kernel(const SweepArgs ar) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   SweepSmem<C> sm(smem_raw);
@@ -528,7 +557,7 @@ __global__ void __launch_bounds__(C::NTHREADS, CTAS_PER_SM) fp_sweep_kernel(cons
   __syncthreads();
   if (wid < C::NWC) {
     reg_alloc<C::CREGS>();
-    consumer_loop<C, NMFP, ECORR>(ar, sm, &s_work, wid, lane);
+    consumer_loop<C, NMFP, ECORR, RES>(ar, sm, &s_work, wid, lane);
   } else {
     reg_dealloc<C::PREGS>();
     producer_loop<C, NMFP, ECORR>(ar, sm, &s_work, wid - C::NWC, lane);
@@ -536,11 +565,11 @@ __global__ void __launch_bounds__(C::NTHREADS, CTAS_PER_SM) fp_sweep_kernel(cons
 }
 
 // ---- launch helpers -------------------------------------------------------------------------
-template <class C, bool NMFP, bool ECORR>
+template <class C, bool NMFP, bool ECORR, bool RES>
 int launch_sweep_cfg(const fastfp_pack* pk, const Group& g, const SweepArgs& base, cudaStream_t st) {
   static bool attr_done[64] = {};
   if (!attr_done[pk->device & 63]) {
-    FFP_CUDA(cudaFuncSetAttribute(fp_sweep_kernel<C, NMFP, ECORR>,
+    FFP_CUDA(cudaFuncSetAttribute(fp_sweep_kernel<C, NMFP, ECORR, RES>,
                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
     attr_done[pk->device & 63] = true;
   }
@@ -554,28 +583,30 @@ int launch_sweep_cfg(const fastfp_pack* pk, const Group& g, const SweepArgs& bas
   const int64_t resident = (int64_t)CTAS_PER_SM * pk->num_sms;
   const unsigned grid = (unsigned)(nwork < resident ? nwork : resident);
   FFP_CUDA(cudaMemsetAsync(a.counter, 0, sizeof(unsigned int), st));
-  fp_sweep_kernel<C, NMFP, ECORR><<<grid, C::NTHREADS, C::SMEM, st>>>(a);
+  fp_sweep_kernel<C, NMFP, ECORR, RES><<<grid, C::NTHREADS, C::SMEM, st>>>(a);
   g_launches += 1;
   FFP_CUDA(cudaGetLastError());
   return 0;
 }
 
-// one translation unit per configuration family instantiates these (compile time)
-int dispatch_sweep_w1(const fastfp_pack*, const Group&, const SweepArgs&, bool nmfp, cudaStream_t);
-int dispatch_sweep_w2(const fastfp_pack*, const Group&, const SweepArgs&, bool nmfp, cudaStream_t);
-int dispatch_sweep_w4(const fastfp_pack*, const Group&, const SweepArgs&, bool nmfp, cudaStream_t);
-int dispatch_sweep_wide(const fastfp_pack*, const Group&, const SweepArgs&, bool nmfp, cudaStream_t);
-int dispatch_sweep_xwide(const fastfp_pack*, const Group&, const SweepArgs&, bool nmfp, cudaStream_t);
+// one translation unit per configuration family instantiates these (compile time); res: the residual-batch mode
+// (diagonal-N, plain-Fp packs only)
+int dispatch_sweep_w1(const fastfp_pack*, const Group&, const SweepArgs&, bool nmfp, bool res, cudaStream_t);
+int dispatch_sweep_w2(const fastfp_pack*, const Group&, const SweepArgs&, bool nmfp, bool res, cudaStream_t);
+int dispatch_sweep_w4(const fastfp_pack*, const Group&, const SweepArgs&, bool nmfp, bool res, cudaStream_t);
+int dispatch_sweep_wide(const fastfp_pack*, const Group&, const SweepArgs&, bool nmfp, bool res, cudaStream_t);
+int dispatch_sweep_xwide(const fastfp_pack*, const Group&, const SweepArgs&, bool nmfp, bool res, cudaStream_t);
 
 #define FFP_SWEEP_CASE(NMBWv, NNBv, WMWv, CIv) FFP_SWEEP_CASE_W(NMBWv, NNBv, WMWv, CIv, 8, 16)
 #define FFP_SWEEP_CASE_W(NMBWv, NNBv, WMWv, CIv, NWCv, NWPv)                                       \
   if (g.cfg.nmbw == NMBWv && g.cfg.nnb == NNBv && g.cfg.wmw == WMWv && g.cfg.ci == CIv &&          \
       g.cfg.nwc == NWCv) {                                                                         \
     using Cfg_ = SweepCfg<NMBWv, NNBv, WMWv, CIv, NWCv, NWPv>;                                      \
-    if (pk->ecorr) return nmfp ? launch_sweep_cfg<Cfg_, true, true>(pk, g, a, st)                   \
-                               : launch_sweep_cfg<Cfg_, false, true>(pk, g, a, st);                 \
-    return nmfp ? launch_sweep_cfg<Cfg_, true, false>(pk, g, a, st)                                 \
-                : launch_sweep_cfg<Cfg_, false, false>(pk, g, a, st);                               \
+    if (res) return launch_sweep_cfg<Cfg_, false, false, true>(pk, g, a, st);                      \
+    if (pk->ecorr) return nmfp ? launch_sweep_cfg<Cfg_, true, true, false>(pk, g, a, st)            \
+                               : launch_sweep_cfg<Cfg_, false, true, false>(pk, g, a, st);          \
+    return nmfp ? launch_sweep_cfg<Cfg_, true, false, false>(pk, g, a, st)                          \
+                : launch_sweep_cfg<Cfg_, false, false, false>(pk, g, a, st);                        \
   }
 
 }  // namespace ffp

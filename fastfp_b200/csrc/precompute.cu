@@ -8,6 +8,9 @@
 // (frequency, pulsar) (fastfp/fastfp.py:81-88). With Sigma = L L^T,
 //   (x|y) = x^T N^-1 y - (G x).(G y)        and       (x|r) = x . w
 // so the per-frequency work collapses to Y = G [s c] plus five weighted dot products.
+#include <algorithm>
+#include <map>
+
 #include "ffp_internal.cuh"
 
 namespace ffp {
@@ -167,6 +170,170 @@ int launch_fp_precompute(fastfp_pack* pk, const double* d_toas, const double* d_
   // caller can ask which pulsar it was (fastfp_pack_factor_info; the Python mirror warns)
   pk->info.assign(P, 0);
   FFP_CUDA(cudaMemcpy(pk->info.data(), pk->d_info, sizeof(int) * P, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+// ---- residual batches (DESIGN.md section 5d) ---------------------------------------------------------
+// R realisations r_k of the residuals enter the sweep only through w_k = C^-1 r_k = r_k / N - G^T (G r_k). Their
+// packets hold, per pulsar, the G rows of the pack and then w_1 .. w_R as rows roundup8(m) .. roundup8(m) + R - 1,
+// laid out for the kernel configuration of roundup8(m) + roundup8(R) rows (its own CI and MP).
+
+// G[j][i] of pulsar pm in the pack's packets
+__device__ __forceinline__ double g_at(const double* packets, const PulsarMeta& pm, int i, int j) {
+  return packets[pm.pk_off + (size_t)(i / pm.ci) * (pm.ci * (4 + pm.mpad)) + 4 * pm.ci +
+                 g_frag_index(i % pm.ci, j, pm.mpad >> 3)];
+}
+
+// One thread per (padded) TOA of the residual layout: (t, 1/N, 0, 0) and the pack's G rows; all other rows zero
+__global__ void res_packets_kernel(double* __restrict__ rpk, const PulsarMeta* __restrict__ rmeta,
+                                   const double* __restrict__ packets, const PulsarMeta* __restrict__ meta) {
+  const PulsarMeta pm = meta[blockIdx.y], rm = rmeta[blockIdx.y];
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  const int CI = rm.ci, mp = rm.mpad;
+  if (i >= rm.nch * CI) return;
+  double* pk = rpk + rm.pk_off + (size_t)(i / CI) * (CI * (4 + mp));
+  const int il = i % CI;
+  const bool valid = i < pm.n;
+  const double* src = packets + pm.pk_off + (size_t)(i / pm.ci) * (pm.ci * (4 + pm.mpad)) + 4 * (i % pm.ci);
+  pk[4 * il] = valid ? src[0] : 0.0;
+  pk[4 * il + 1] = valid ? src[1] : 0.0;
+  pk[4 * il + 2] = 0.0;  // the producers' s.w, c.w are not used in this mode
+  pk[4 * il + 3] = 0.0;
+  double* gp = pk + 4 * CI;
+  for (int j = 0; j < mp; ++j) gp[g_frag_index(il, j, mp >> 3)] = valid && j < pm.m ? g_at(packets, pm, i, j) : 0.0;
+}
+
+// U[p][k][j] = sum_i G[j][i] r_k[i] for 8 rows x 32 realisations per CTA, TOAs staged 32 at a time. Each entry is
+// summed by one thread in a fixed order (32-TOA partial sums, then their running total), so its bits do not depend
+// on where its realisation sits in the batch.
+__global__ void __launch_bounds__(256) ur_batch_kernel(const double* __restrict__ packets,
+                                                       const PulsarMeta* __restrict__ meta,
+                                                       const double* __restrict__ res, int R, int ld,
+                                                       double* __restrict__ U) {
+  const PulsarMeta pm = meta[blockIdx.z];
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const int j0 = blockIdx.x * 8, k0 = blockIdx.y * 32;
+  if (j0 >= pm.m) return;
+  __shared__ double Gs[8][32];
+  __shared__ double Rs[32][33];
+  const double* rp = res + (size_t)R * pm.raw_off;
+  double acc = 0.0;
+  for (int i0 = 0; i0 < pm.n; i0 += 32) {
+    const int i = i0 + tx;
+    Gs[ty][tx] = i < pm.n && j0 + ty < pm.m ? g_at(packets, pm, i, j0 + ty) : 0.0;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int kk = ty + 8 * q;
+      Rs[kk][tx] = i < pm.n && k0 + kk < R ? rp[(size_t)(k0 + kk) * pm.n + i] : 0.0;
+    }
+    __syncthreads();
+    double part = 0.0;
+#pragma unroll 8
+    for (int ii = 0; ii < 32; ++ii) part = fma(Gs[ty][ii], Rs[tx][ii], part);
+    acc += part;
+    __syncthreads();
+  }
+  if (j0 + ty < pm.m && k0 + tx < R) U[((size_t)blockIdx.z * R + k0 + tx) * ld + j0 + ty] = acc;
+}
+
+// w_k[i] = r_k[i] / N_i - sum_j G[j][i] U[k][j] (w_kernel's order) for 32 TOAs x 8 realisations per CTA, written
+// straight into the residual packets: a warp takes 4 TOAs x 8 rows, i.e. one 256-byte A fragment.
+__global__ void __launch_bounds__(256) w_batch_kernel(double* __restrict__ rpk, const PulsarMeta* __restrict__ rmeta,
+                                                      const double* __restrict__ packets,
+                                                      const PulsarMeta* __restrict__ meta,
+                                                      const double* __restrict__ res, int R, int ld,
+                                                      const double* __restrict__ U) {
+  const PulsarMeta pm = meta[blockIdx.z], rm = rmeta[blockIdx.z];
+  const int lane = threadIdx.x & 31, wq = threadIdx.x >> 5;
+  const int i0 = blockIdx.x * 32, k0 = blockIdx.y * 8;
+  if (i0 >= pm.n) return;
+  __shared__ double Gs[32][33];
+  __shared__ double Us[8][33];
+  const int il = 4 * wq + (lane & 3), kl = lane >> 2;
+  const int i = i0 + il, k = k0 + kl;
+  const double* Up = U + (size_t)blockIdx.z * R * ld;
+  double acc = 0.0;
+  for (int j0 = 0; j0 < pm.m; j0 += 32) {
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int jj = wq + 8 * q;
+      Gs[jj][lane] = i0 + lane < pm.n && j0 + jj < pm.m ? g_at(packets, pm, i0 + lane, j0 + jj) : 0.0;
+    }
+    Us[wq][lane] = k0 + wq < R && j0 + lane < pm.m ? Up[(size_t)(k0 + wq) * ld + j0 + lane] : 0.0;
+    __syncthreads();
+    const int jn = pm.m - j0 < 32 ? pm.m - j0 : 32;
+    for (int jj = 0; jj < jn; ++jj) acc = fma(Gs[jj][il], Us[kl][jj], acc);
+    __syncthreads();
+  }
+  if (i >= pm.n || k >= R) return;
+  const double ninv = packets[pm.pk_off + (size_t)(i / pm.ci) * (pm.ci * (4 + pm.mpad)) + 4 * (i % pm.ci) + 1];
+  const double w = res[(size_t)R * pm.raw_off + (size_t)k * pm.n + i] * ninv - acc;
+  const int CI = rm.ci;
+  rpk[rm.pk_off + (size_t)(i / CI) * (CI * (4 + rm.mpad)) + 4 * CI +
+      g_frag_index(i % CI, ((pm.m + 7) & ~7) + k, rm.mpad >> 3)] = w;
+}
+
+void res_release(fastfp_pack* pk) {
+  for (auto& g : pk->res_groups) cudaFree(g.d_pidx);
+  pk->res_groups.clear();
+  cudaFree(pk->d_res_packets);
+  cudaFree(pk->d_res_meta);
+  cudaFree(pk->d_res_terms);
+  pk->d_res_packets = nullptr;
+  pk->d_res_meta = nullptr;
+  pk->d_res_terms = nullptr;
+  pk->res_terms_cap = 0;
+  pk->res_R = 0;
+  pk->res_bytes = 0;
+}
+
+int build_res_packets(fastfp_pack* pk, int64_t R, const double* d_res, cudaStream_t st) {
+  const int P = pk->P;
+  std::vector<PulsarMeta> rmeta = pk->meta;
+  std::map<KernelCfg, std::vector<int>> groups;
+  int64_t off = 0;
+  int mmax = 0, nmax = 0, npad = 0;
+  for (int p = 0; p < P; ++p) {
+    PulsarMeta& rm = rmeta[p];
+    KernelCfg kc{};
+    if (!sweep_config((rm.m + 7) / 8 * 8 + (int)(R + 7) / 8 * 8, &kc)) {
+      set_error("residual batch: no kernel configuration for pulsar " + std::to_string(p));
+      return -3;
+    }
+    rm.ci = kc.ci;
+    rm.nch = (rm.n + kc.ci - 1) / kc.ci;
+    rm.mpad = kc.mp();
+    rm.pk_off = off;
+    off += (int64_t)rm.nch * rm.ci * (4 + rm.mpad);
+    groups[kc].push_back(p);
+    mmax = std::max(mmax, rm.m);
+    nmax = std::max(nmax, rm.n);
+    npad = std::max(npad, rm.nch * rm.ci);
+  }
+  FFP_CUDA(cudaMalloc(&pk->d_res_meta, sizeof(PulsarMeta) * P));
+  FFP_CUDA(cudaMemcpy(pk->d_res_meta, rmeta.data(), sizeof(PulsarMeta) * P, cudaMemcpyHostToDevice));
+  FFP_CUDA(cudaMalloc(&pk->d_res_packets, (size_t)off * 8));
+  for (auto& kv : groups) {
+    Group g;
+    g.cfg = kv.first;
+    g.count = (int)kv.second.size();
+    FFP_CUDA(cudaMalloc(&g.d_pidx, sizeof(int) * g.count));
+    pk->res_groups.push_back(g);
+    FFP_CUDA(cudaMemcpy(g.d_pidx, kv.second.data(), sizeof(int) * g.count, cudaMemcpyHostToDevice));
+  }
+  pk->res_bytes = off * 8 + (int64_t)sizeof(PulsarMeta) * P;
+  DeviceBuf<double> U;
+  FFP_CUDA(dev_alloc(&U, (size_t)P * R * mmax));
+  res_packets_kernel<<<dim3((npad + 127) / 128, P), 128, 0, st>>>(pk->d_res_packets, pk->d_res_meta, pk->d_packets,
+                                                                  pk->d_meta);
+  ur_batch_kernel<<<dim3((mmax + 7) / 8, (unsigned)((R + 31) / 32), P), 256, 0, st>>>(pk->d_packets, pk->d_meta, d_res,
+                                                                                     (int)R, mmax, U.get());
+  w_batch_kernel<<<dim3((nmax + 31) / 32, (unsigned)((R + 7) / 8), P), 256, 0, st>>>(
+      pk->d_res_packets, pk->d_res_meta, pk->d_packets, pk->d_meta, d_res, (int)R, mmax, U.get());
+  g_launches += 3;
+  FFP_CUDA(cudaGetLastError());
+  FFP_CUDA(cudaStreamSynchronize(st));  // U and the caller's staging buffer are released on return
+  pk->res_R = R;
   return 0;
 }
 

@@ -152,6 +152,36 @@ class _PackCache:
         return run(self._ensure(lists, key=key))  # the inputs changed: rebuild, repeat
 
 
+def _tile_cost(rows: int) -> float:
+    """Modelled cost of one residual pass per (frequency, TOA): the padded width MP that ``sweep_config`` gives ``rows`` G
+    rows, times a per-row factor. On an H100 a tile row costs about the same in every configuration measured (0.49-0.51
+    ms per row at C2 shapes for 40 to 384 rows) except the 8-frequency family with 10 row blocks per warp (640 rows),
+    which costs 1.3-1.5 times as much per row (DESIGN.md section 5d). That family was measured at 6 row blocks (384
+    rows, no extra cost) and at 10; the 7 to 9 blocks in between were not measured and are given the 10-block factor."""
+    for top, per_block in ((40, 8), (80, 8), (160, 16), (320, 32), (640, 64)):
+        if rows <= top:
+            nmbw = -(-rows // per_block)
+            return nmbw * per_block * (1.4 if top == 640 and nmbw >= 7 else 1.0)
+    raise ValueError(f"{rows} rows exceed the sweep kernel")
+
+
+def batch_pass_rows(R: int, m) -> int:
+    """Realisations per pass of :meth:`FastFp.calculate_Fp_batch` for ``R`` realisations of pulsars of basis widths
+    ``m``: of the even splits of ``R`` into passes the library takes (at most ``_cabi.max_residual_rows`` rows each),
+    the one with the least modelled cost, passes x :func:`_tile_cost` of ``roundup8(max m) + roundup8(rows)`` rows;
+    among equal costs the fewest passes."""
+    mr = -(-max(m) // 8) * 8
+    rmax = _cabi.max_residual_rows(m)
+    best = None
+    for cap in sorted({min(R, rmax)} | set(range(8, min(R, rmax), 8))):
+        npass = -(-R // cap)
+        rows = -(-R // npass)
+        cost = npass * _tile_cost(mr + -(-rows // 8) * 8)
+        if best is None or (cost, npass) < best[:2]:
+            best = (cost, npass, rows)
+    return best[2]
+
+
 def _is_cuda_tensor(x) -> bool:
     return type(x).__module__.startswith("torch") and getattr(x, "is_cuda", False)
 
@@ -209,6 +239,73 @@ class FastFp(_PackCache):
         return np.float64(res[0]) if f.ndim == 0 else res.reshape(f.shape)
 
     compute_Fp = calculate_Fp
+
+    def calculate_Fp_batch(self, fgw, Nvecs, Ts, sigmas, residuals):
+        """Fp at ``fgw`` for each of ``R`` realisations of the residuals (simulated noise for a false-alarm
+        calibration, injected signals for a detection study), with the pulsars, noise model and basis of
+        ``Nvecs, Ts, sigmas``. ``residuals`` is a list of ``P`` arrays of shape ``(R, n_p)``; row ``k`` of the result
+        is the Fp :meth:`calculate_Fp` gives with residuals ``residuals[p][k]``: ``(R,)`` for a scalar ``fgw``,
+        ``(R, *fgw.shape)`` for an array, a CUDA tensor on torch's current stream for a float64 CUDA tensor (so
+        ``parallel.sharded_sweep(..., lead_shape=(R,))`` spreads it over several GPUs).
+
+        The realisations ride along as extra rows of the fp64 sweep kernel (``fastfp_fp_sweep_residuals``, whatever
+        ``path`` says). Values meet the parity bar of :meth:`calculate_Fp` but are not bit-identical to it. The set is
+        cached on the pack and uploaded again when any byte of ``residuals`` changes. A set of several passes is
+        uploaded pass by pass on every call, and each upload synchronises the stream, so with a CUDA-tensor ``fgw``
+        such a call returns only when its last pass has been launched and is not asynchronous; the content hash of
+        ``residuals`` is also taken on the calling thread before the first launch. The library takes at most ``_cabi.max_residual_rows`` rows per pass (568
+        at m = 72); ``R`` is split into passes of :func:`batch_pass_rows` rows, the split with the least modelled
+        sweep cost (measured per-row costs of the kernel configurations). The pass size selects the kernel configuration, so values can differ in the last bits
+        between different ``R``; within one ``R`` every row is computed alike wherever it sits."""
+        res = [_cabi.as_f64(r) for r in residuals]
+        if len(res) != len(self.toas):
+            raise ValueError(f"residuals must be a list of {len(self.toas)} arrays (one per pulsar)")
+        R = res[0].shape[0] if res[0].ndim == 2 else -1
+        for p, r in enumerate(res):
+            if r.shape != (R, self.toas[p].shape[0]):
+                raise ValueError(f"residuals[{p}] must have shape (R, {self.toas[p].shape[0]}) with the same R >= 1 for "
+                                 f"every pulsar; got {r.shape}")
+        if R < 1:
+            raise ValueError("residuals must hold at least one realisation")
+        lists = (Nvecs, Ts, sigmas)
+        res_key = _fingerprint([res])
+
+        def passes(pack, stream=0):
+            rows = batch_pass_rows(R, pack.m)
+            for lo in range(0, R, rows):
+                hi = min(R, lo + rows)
+                key = (res_key, lo, hi)
+                if self._res_pack is not pack or self._res_key != key:
+                    self._res_pack, self._res_key = None, None
+                    pack.set_residuals([r[lo:hi] for r in res], stream=stream)
+                    self._res_pack, self._res_key = pack, key
+                yield lo, hi
+
+        if _is_cuda_tensor(fgw):
+            import torch
+
+            f, stream = self._device_freqs(fgw)
+            out = torch.empty((R, f.shape[0]), dtype=torch.float64, device=f.device)
+
+            def run(pack):
+                for lo, _ in passes(pack, stream):
+                    pack.fp_sweep_residuals((f.data_ptr(), f.shape[0]), out=out[lo].data_ptr(), stream=stream)
+                return out
+
+            return self._run_verified(lists, run, asynchronous=True).reshape((R,) + tuple(fgw.shape))
+        f = np.asarray(fgw, dtype=np.float64)
+        fl = f.reshape(-1)
+
+        def run(pack):
+            out = np.empty((R, fl.shape[0]))
+            for lo, hi in passes(pack):
+                pack.fp_sweep_residuals(fl, out=out[lo:hi])
+            return out
+
+        return self._run_verified(lists, run, asynchronous=False).reshape((R,) + f.shape)
+
+    _res_pack = None
+    _res_key = None
 
     def per_pulsar_terms(self, fgw, Nvecs, Ts, sigmas):
         """``0.5 * N^T M^-1 N`` per pulsar, ``(P, F)`` -- the summands of ``fastfp.py:90``."""

@@ -120,6 +120,31 @@ int fastfp_fe_sweep(const fastfp_pack_t* pack, const double* freqs, int64_t F, c
 int fastfp_fe_skymax(const fastfp_pack_t* pack, const double* freqs, int64_t F, const double* fplus,
                      const double* fcross, int64_t S, double* fe_max, int64_t* sky_index, int flags, void* stream);
 
+/* ---- Fp of a batch of residual realisations ---------------------------------------------------------------
+ * False-alarm calibration on simulated noise and injection-recovery studies need Fp over one frequency grid for R
+ * residual vectors of the same pulsars, noise model and basis. The residuals enter only through w = C^-1 r, so the R
+ * realisations ride along as R extra rows of the G tiles the fp64 kernel already streams, and the sin/cos work is
+ * shared (DESIGN.md section 5d).
+ * fastfp_pack_set_residuals: residuals[p] is a host array (R, n_p) row-major. The pack keeps the realisations'
+ *   packets until the next call or fastfp_pack_destroy; R == 0 releases them. fastfp_pack_bytes counts them. Each
+ *   pulsar then needs roundup8(m_p) + roundup8(R) rows of the kernel's 640, so R <= 640 - roundup8(max_p m_p)
+ *   (568 at m = 72). Returns FASTFP_ERR_INVALID for a NULL pack or array, R < 0 or an nmfp pack, and
+ *   FASTFP_ERR_UNSUPPORTED for a block-N pack or an R above the limit (the message names the limit and the widest
+ *   pulsar). While it runs the call also holds a device staging copy of the realisations, R * sum_p n_p doubles
+ *   (3.1 GB at R = 568 for 68 pulsars of 10^4 TOAs), on top of the packets it keeps (sum_p ceil(n_p / CI) * CI *
+ *   (4 + MP) doubles, 3.5 GB in that case); the staging copy is freed before it returns.
+ * fastfp_fp_sweep_residuals: out is (R, F) row-major, out[k*F + f] = the Fp fastfp_fp_sweep returns for a pack
+ *   built with residuals r_k (pulsar sum in pulsar order from 0, same 2x2 rule). The values meet the same parity bar
+ *   as fastfp_fp_sweep but are not bit-identical to it: (s|r_k), (c|r_k) come from the MMA instead of the producers'
+ *   dot products. It always runs the fp64 DMMA kernel, whatever fastfp_pack_path says. flags as for
+ *   fastfp_fp_sweep. FASTFP_ERR_INVALID if no realisations are set; F == 0 writes nothing.
+ *   Device scratch: the terms of one frequency batch, R * P * F_batch doubles with F_batch = max(1024,
+ *   min(F, 2^27 / (R * P))) (at most 1 GiB unless R * P > 131 072), kept until the realisations are replaced or
+ *   released, plus R * F doubles for host outputs in the pack's output buffer, kept until fastfp_pack_destroy. */
+int fastfp_pack_set_residuals(fastfp_pack_t* pack, int64_t R, const double* const* residuals, void* stream);
+int fastfp_fp_sweep_residuals(const fastfp_pack_t* pack, const double* freqs, int64_t F, double* out, int flags,
+                              void* stream);
+
 /* ---- noise-marginalised Fp -----------------------------------------------------------
  * fastfp_nmfp_pack_create: NMFP.__init__ (fastfp/nmfp.py:45-51) plus the (TNTs, Nvecs, Ts)
  * of get_mats_nmfp (fastfp/utils.py:97-101). Sigma_d = TNT + diag(phiinv_d) is formed per
