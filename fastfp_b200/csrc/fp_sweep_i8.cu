@@ -472,6 +472,10 @@ __global__ void __launch_bounds__(THREADS, 1) fp_sweep_i8_kernel(const Args ar) 
             if (ar.inner) {
               double* o = ar.inner + ((size_t)p * ar.F + fidx) * 5;
               o[0] = a[0] - b[0]; o[1] = a[1] - b[1]; o[2] = a[2] - b[2]; o[3] = N0; o[4] = N1;
+              if (!(ar.freqs[fidx] > 0.0)) {  // f <= 0: NaN like f**(1/3) (Fe is even in f)
+#pragma unroll
+                for (int k = 0; k < 5; ++k) o[k] = __longlong_as_double(0x7ff8000000000000LL);
+              }
             }
           }
         }

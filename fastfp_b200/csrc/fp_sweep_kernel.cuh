@@ -515,6 +515,11 @@ __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>&
         if (ar.inner) {  // the inner products themselves (no f^(-1/3) prefactor: it cancels in every statistic)
           double* o = ar.inner + ((size_t)p * ar.F + fidx) * 5;
           o[0] = a[0] - b[0]; o[1] = a[1] - b[1]; o[2] = a[2] - b[2]; o[3] = a[3]; o[4] = a[4];
+          // f <= 0: NaN like f**(1/3). Fe is even in f (s flips sign), so without this f < 0 would give Fe(|f|)
+          if (!(sm.fq[tid] > 0.0)) {
+#pragma unroll
+            for (int k = 0; k < 5; ++k) o[k] = __longlong_as_double(0x7ff8000000000000LL);
+          }
         }
       }
     }

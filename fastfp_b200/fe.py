@@ -40,7 +40,8 @@ class FastFe(FastFp):
 
     def calculate_Fe(self, fgw, gwtheta, gwphi, Nvecs, Ts, sigmas):
         """Fe at frequency ``fgw`` (scalar or ``(F,)``, host array or CUDA tensor) and sky position(s)
-        ``gwtheta``, ``gwphi`` (scalars or ``(S,)``): returns a scalar, ``(F,)``, ``(S,)`` or ``(S, F)``."""
+        ``gwtheta``, ``gwphi`` (scalars or ``(S,)``): returns a scalar, ``(F,)``, ``(S,)`` or ``(S, F)``. A frequency
+        ``f <= 0`` gives NaN, as in :meth:`calculate_Fp` (the reference's ``f^(-1/3)``)."""
         th, ph = np.asarray(gwtheta, dtype=np.float64), np.asarray(gwphi, dtype=np.float64)
         sky_batched = th.ndim > 0 or ph.ndim > 0
         th, ph = np.broadcast_arrays(np.atleast_1d(th), np.atleast_1d(ph))

@@ -101,7 +101,8 @@ int fastfp_fp_terms(const fastfp_pack_t* pack, const double* freqs, int64_t F, d
  * per-(pulsar, frequency) inner products as Fp (fastfp/fastfp.py:81-88): with antenna patterns F+_p, Fx_p
  *   N = sum_p [F+ N_p ; Fx N_p],  M = sum_p [[F+^2 M_p, F+Fx M_p],[F+Fx M_p, Fx^2 M_p]],  Fe = 1/2 N^T M^-1 N
  * (N_p, M_p as in fastfp.py:83-88; 4x4 general solve with partial pivoting). fplus, fcross: host arrays (S, P)
- * row-major; out: (S, F) row-major. flags as for fastfp_fp_sweep. One sweep + one combine kernel per call. */
+ * row-major; out: (S, F) row-major. flags as for fastfp_fp_sweep. One sweep + one combine kernel per call.
+ * f <= 0 gives NaN at every sky position, as for Fp (the reference's f^(-1/3)). */
 int fastfp_fe_sweep(const fastfp_pack_t* pack, const double* freqs, int64_t F, const double* fplus,
                     const double* fcross, int64_t S, double* out, int flags, void* stream);
 

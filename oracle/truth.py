@@ -45,18 +45,14 @@ def _fwd_ld(L, B):
     return X
 
 
-def fp_sweep_truth(freqs, toas, residuals, Nvecs, Ts, sigmas, chunk=128):
-    """Truth for ``fp_sweep``. Returns ``(terms (P,F) longdouble, cond (P,F) float64)``.
-
-    ``cond[p, f]`` bounds (to first order, in units of the relative rounding error committed
-    in each of the two cancelling parts of every inner product) the absolute change of the
-    per-pulsar term ``0.5 * N^T M^-1 N``:
-    ``|x|^T A + 0.5 |x|^T B |x|`` with ``x = M^-1 N`` and ``A_k``/``B_kl`` the sums of the
-    magnitudes of the two parts of ``N_k``/``M_kl``."""
+def sweep_inner_truth(freqs, toas, residuals, Nvecs, Ts, sigmas, chunk=128):
+    """The five per-(pulsar, frequency) inner products of the sweep, ``(P, F)`` longdouble each: ``Mss, Msc, Mcc``
+    = (s|s), (s|c), (c|c) and ``Ns, Nc`` = (s|r), (c|r), plus the magnitudes of their two cancelling parts (the
+    diagonal-N part and the subtracted Woodbury part), ``A0, A1`` for ``Ns, Nc`` and ``B00, B01, B11`` for the
+    three entries of M. :func:`fp_sweep_truth` and :func:`fe_truth` are formed from them."""
     freqs = np.atleast_1d(np.asarray(freqs, dtype=np.float64))
     F, P = freqs.shape[0], len(toas)
-    terms = np.zeros((P, F), dtype=LD)
-    cond = np.zeros((P, F))
+    out = {k: np.zeros((P, F), dtype=LD) for k in _INNER_KEYS}
     for p in range(P):
         toa = np.asarray(toas[p], dtype=np.float64)
         ninv = LD(1) / np.asarray(Nvecs[p], dtype=LD)
@@ -77,19 +73,42 @@ def fp_sweep_truth(freqs, toas, residuals, Nvecs, Ts, sigmas, chunk=128):
             sNr, cNr = S @ rn, C @ rn
             bss, bsc, bcc = (US * US).sum(1), (US * UC).sum(1), (UC * UC).sum(1)
             bsr, bcr = US @ ur, UC @ ur
-            Mss, Msc, Mcc = sNs - bss, sNc - bsc, cNc - bcc
-            Ns, Nc = sNr - bsr, cNr - bcr
-            det = Mss * Mcc - Msc * Msc
-            x0 = (Mcc * Ns - Msc * Nc) / det
-            x1 = (Mss * Nc - Msc * Ns) / det
-            terms[p, lo : lo + chunk] = LD(0.5) * (Ns * x0 + Nc * x1)
-            A0 = np.abs(sNr) + np.abs(bsr)
-            A1 = np.abs(cNr) + np.abs(bcr)
-            B00, B01, B11 = sNs + bss, np.abs(sNc) + np.abs(bsc), cNc + bcc
-            ax0, ax1 = np.abs(x0), np.abs(x1)
-            c = ax0 * A0 + ax1 * A1 + LD(0.5) * (ax0 * ax0 * B00 + 2 * ax0 * ax1 * B01 + ax1 * ax1 * B11)
-            cond[p, lo : lo + chunk] = c.astype(np.float64)
-    return terms, cond
+            _store(out, p, slice(lo, lo + chunk), Mss=sNs - bss, Msc=sNc - bsc, Mcc=cNc - bcc, Ns=sNr - bsr,
+                   Nc=cNr - bcr, A0=np.abs(sNr) + np.abs(bsr), A1=np.abs(cNr) + np.abs(bcr), B00=sNs + bss,
+                   B01=np.abs(sNc) + np.abs(bsc), B11=cNc + bcc)
+    return out
+
+
+_INNER_KEYS = ("Mss", "Msc", "Mcc", "Ns", "Nc", "A0", "A1", "B00", "B01", "B11")
+
+
+def _store(out, p, cols, **vals):
+    for k, v in vals.items():
+        out[k][p, cols] = v
+
+
+def terms_truth(inner):
+    """``(terms (P,F) longdouble, cond (P,F) float64)`` of :func:`fp_sweep_truth` from :func:`sweep_inner_truth`."""
+    Mss, Msc, Mcc, Ns, Nc = (inner[k] for k in ("Mss", "Msc", "Mcc", "Ns", "Nc"))
+    det = Mss * Mcc - Msc * Msc
+    x0 = (Mcc * Ns - Msc * Nc) / det
+    x1 = (Mss * Nc - Msc * Ns) / det
+    terms = LD(0.5) * (Ns * x0 + Nc * x1)
+    A0, A1, B00, B01, B11 = (inner[k] for k in ("A0", "A1", "B00", "B01", "B11"))
+    ax0, ax1 = np.abs(x0), np.abs(x1)
+    c = ax0 * A0 + ax1 * A1 + LD(0.5) * (ax0 * ax0 * B00 + 2 * ax0 * ax1 * B01 + ax1 * ax1 * B11)
+    return terms, c.astype(np.float64)
+
+
+def fp_sweep_truth(freqs, toas, residuals, Nvecs, Ts, sigmas, chunk=128):
+    """Truth for ``fp_sweep``. Returns ``(terms (P,F) longdouble, cond (P,F) float64)``.
+
+    ``cond[p, f]`` bounds (to first order, in units of the relative rounding error committed
+    in each of the two cancelling parts of every inner product) the absolute change of the
+    per-pulsar term ``0.5 * N^T M^-1 N``:
+    ``|x|^T A + 0.5 |x|^T B |x|`` with ``x = M^-1 N`` and ``A_k``/``B_kl`` the sums of the
+    magnitudes of the two parts of ``N_k``/``M_kl``."""
+    return terms_truth(sweep_inner_truth(freqs, toas, residuals, Nvecs, Ts, sigmas, chunk))
 
 
 def get_xCy_truth(Nvec, T, sigma, x, y):
@@ -120,10 +139,14 @@ def fp_sweep_truth_blockn(freqs, toas, residuals, blocks, Ts, phiinvs=None, chun
     where both run. ``blocks[p]`` is ``(nvec, [(start, stop), ...], jvec)``. With ``sigmas`` given, those
     float64 matrices are taken as exact inputs (what the engine is handed), like :func:`fp_sweep_truth` does;
     otherwise ``Sigma`` is formed here from ``phiinvs``. Returns ``(terms, cond)`` like :func:`fp_sweep_truth`."""
+    return terms_truth(sweep_inner_truth_blockn(freqs, toas, residuals, blocks, Ts, phiinvs, chunk, sigmas))
+
+
+def sweep_inner_truth_blockn(freqs, toas, residuals, blocks, Ts, phiinvs=None, chunk=64, sigmas=None):
+    """:func:`sweep_inner_truth` for a block-diagonal N (arguments as :func:`fp_sweep_truth_blockn`)."""
     freqs = np.atleast_1d(np.asarray(freqs, dtype=np.float64))
     F, P = freqs.shape[0], len(toas)
-    terms = np.zeros((P, F), dtype=LD)
-    cond = np.zeros((P, F))
+    out = {k: np.zeros((P, F), dtype=LD) for k in _INNER_KEYS}
     for p in range(P):
         toa = np.asarray(toas[p], dtype=np.float64)
         nvec, slices, jvec = blocks[p]
@@ -170,19 +193,81 @@ def fp_sweep_truth_blockn(freqs, toas, residuals, blocks, Ts, phiinvs=None, chun
             sNr, cNr = S @ rn, C @ rn
             bss, bsc, bcc = (US * US).sum(1), (US * UC).sum(1), (UC * UC).sum(1)
             bsr, bcr = US @ ur, UC @ ur
-            Mss, Msc, Mcc = sNs - bss, sNc - bsc, cNc - bcc
-            Ns, Nc = sNr - bsr, cNr - bcr
-            det = Mss * Mcc - Msc * Msc
-            x0 = (Mcc * Ns - Msc * Nc) / det
-            x1 = (Mss * Nc - Msc * Ns) / det
-            terms[p, lo : lo + chunk] = LD(0.5) * (Ns * x0 + Nc * x1)
             # conditioning: the diagonal-N part and the two subtracted parts (epoch correction, Woodbury)
             dS, dC = S * ninv, C * ninv
             pss, psc, pcc = (S * dS).sum(1), np.abs(S * dC).sum(1), (C * dC).sum(1)
-            A0 = np.abs(S * (r * ninv)).sum(1) + np.abs(bsr)
-            A1 = np.abs(C * (r * ninv)).sum(1) + np.abs(bcr)
-            B00, B01, B11 = 2 * pss - sNs + bss, psc + np.abs(bsc), 2 * pcc - cNc + bcc
-            ax0, ax1 = np.abs(x0), np.abs(x1)
-            c = ax0 * A0 + ax1 * A1 + LD(0.5) * (ax0 * ax0 * B00 + 2 * ax0 * ax1 * B01 + ax1 * ax1 * B11)
-            cond[p, lo : lo + chunk] = c.astype(np.float64)
-    return terms, cond
+            _store(out, p, slice(lo, lo + chunk), Mss=sNs - bss, Msc=sNc - bsc, Mcc=cNc - bcc, Ns=sNr - bsr,
+                   Nc=cNr - bcr, A0=np.abs(S * (r * ninv)).sum(1) + np.abs(bsr),
+                   A1=np.abs(C * (r * ninv)).sum(1) + np.abs(bcr), B00=2 * pss - sNs + bss, B01=psc + np.abs(bsc),
+                   B11=2 * pcc - cNc + bcc)
+    return out
+
+
+def _solve_ld(M, b):
+    """``M^-1 b`` for a batch of small systems, ``M (K, n, n)``, ``b (K, n)``, in longdouble (NumPy's LAPACK-backed
+    solve has no longdouble): Gaussian elimination with partial pivoting, then back substitution."""
+    A, y = np.array(M, dtype=LD), np.array(b, dtype=LD)
+    K, n = y.shape
+    ar = np.arange(K)
+    for c in range(n):
+        piv = c + np.argmax(np.abs(A[:, c:, c]), axis=1)
+        A[ar, c], A[ar, piv] = A[ar, piv], A[ar, c].copy()
+        y[ar, c], y[ar, piv] = y[ar, piv], y[ar, c].copy()
+        for r in range(c + 1, n):
+            l = A[:, r, c] / A[:, c, c]
+            A[:, r, c:] -= l[:, None] * A[:, c, c:]
+            y[:, r] -= l * y[:, c]
+    x = np.zeros_like(y)
+    for r in range(n - 1, -1, -1):
+        x[:, r] = (y[:, r] - (A[:, r, r + 1 :] * x[:, r + 1 :]).sum(1)) / A[:, r, r]
+    return x
+
+
+def fe_truth_from_inner(inner, freqs, fplus, fcross):
+    """The Fe-statistic ``0.5 N^T M^-1 N`` of ``S`` sky positions (antenna patterns ``fplus``, ``fcross``: ``(S, P)``)
+    from the per-pulsar inner products of :func:`sweep_inner_truth`: returns ``(fe (S,F) longdouble, cond (S,F)
+    float64)``, NaN at ``f <= 0`` (the ``f^(-1/3)`` prefactor of the reference convention).
+
+    With the four templates ``[F+ s, F+ c, Fx s, Fx c]`` of every pulsar, ``N = sum_p [F+ N_p ; Fx N_p]`` and
+    ``M = sum_p [[F+^2 M_p, F+ Fx M_p], [F+ Fx M_p, Fx^2 M_p]]``. ``cond`` generalises the figure of
+    :func:`fp_sweep_truth`: ``|x|^T A + 0.5 |x|^T B |x|`` with ``x = M^-1 N``, ``A = sum_p [|F+| A_p ; |Fx| A_p]`` and
+    ``B = sum_p [[F+^2 B_p, |F+ Fx| B_p], [|F+ Fx| B_p, Fx^2 B_p]]`` over the part magnitudes ``A_p``, ``B_p``."""
+    freqs = np.atleast_1d(np.asarray(freqs, dtype=np.float64))
+    fp, fx = np.asarray(fplus, dtype=LD), np.asarray(fcross, dtype=LD)
+    S, F = fp.shape[0], freqs.shape[0]
+    pp, px, xx = fp * fp, fp * fx, fx * fx
+    g = {k: inner[k] for k in _INNER_KEYS}
+    N = np.stack((fp @ g["Ns"], fp @ g["Nc"], fx @ g["Ns"], fx @ g["Nc"]), axis=-1)  # (S, F, 4)
+
+    def quad(a, b, c, w_pp, w_px, w_xx):  # sum_p of the 4x4 weighting of the symmetric 2x2 [[a, b], [b, c]]
+        m = np.empty((S, F, 4, 4), dtype=LD)
+        for (i, j), w in (((0, 0), w_pp), ((0, 2), w_px), ((2, 0), w_px), ((2, 2), w_xx)):
+            m[..., i, j], m[..., i, j + 1] = w @ a, w @ b
+            m[..., i + 1, j], m[..., i + 1, j + 1] = w @ b, w @ c
+        return m
+
+    M = quad(g["Mss"], g["Msc"], g["Mcc"], pp, px, xx)
+    with np.errstate(all="ignore"):
+        x = _solve_ld(M.reshape(-1, 4, 4), N.reshape(-1, 4)).reshape(S, F, 4)
+        fe = LD(0.5) * (N * x).sum(-1)
+        afp, afx = np.abs(fp), np.abs(fx)
+        A = np.stack((afp @ g["A0"], afp @ g["A1"], afx @ g["A0"], afx @ g["A1"]), axis=-1)
+        B = quad(g["B00"], g["B01"], g["B11"], pp, np.abs(px), xx)
+        ax = np.abs(x)
+        cond = (ax * A).sum(-1) + LD(0.5) * np.einsum("sfk,sfkl,sfl->sf", ax, B, ax)
+    bad = ~(freqs > 0)
+    fe[:, bad] = np.nan
+    cond[:, bad] = np.nan
+    return fe, cond.astype(np.float64)
+
+
+def fe_truth(freqs, fplus, fcross, toas, residuals, Nvecs, Ts, sigmas, blocks=None):
+    """Truth for ``fastfp_fe_sweep``: ``(fe (S,F) longdouble, cond (S,F) float64)`` for the antenna patterns
+    ``fplus``, ``fcross`` ``(S, P)`` (:func:`fe_truth_from_inner`). The inner products are those of
+    :func:`fp_sweep_truth`; with ``blocks`` (as in :func:`fp_sweep_truth_blockn`, ``Nvecs`` then unused) ``N^-1`` is
+    applied by Sherman-Morrison and ``sigmas`` are the exact block-N Sigma matrices."""
+    if blocks is None:
+        inner = sweep_inner_truth(freqs, toas, residuals, Nvecs, Ts, sigmas)
+    else:
+        inner = sweep_inner_truth_blockn(freqs, toas, residuals, blocks, Ts, sigmas=sigmas)
+    return fe_truth_from_inner(inner, freqs, fplus, fcross)

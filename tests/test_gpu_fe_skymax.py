@@ -142,8 +142,9 @@ def test_ties_and_nan():
     # no position has a value: (NaN, -1) at every frequency, and at the frequencies where the map is all NaN
     v, i = pack.fe_skymax(freqs, Z, Z)
     assert np.isnan(v).all() and (i == -1).all()
-    assert np.isnan(zmap[:, -2]).all()  # f = 0
-    assert np.isnan(got[0][-2]) and got[1][-2] == -1
+    for k in (-2, -1):  # f = 0 and f < 0
+        assert np.isnan(zmap[:, k]).all() and np.isnan(base[0][k]) and base[1][k] == -1
+        assert np.isnan(got[0][k]) and got[1][k] == -1
 
 
 def test_device_resident_calls():
