@@ -40,6 +40,8 @@ SYMBOLS = {
                                    C.c_void_p, C.c_int, C.c_void_p]),
     "fastfp_pack_set_residuals": (C.c_int, [C.c_void_p, C.c_int64, c_double_pp, C.c_void_p]),
     "fastfp_fp_sweep_residuals": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p]),
+    "fastfp_fe_skymax_residuals": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
+                                             C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     "fastfp_nmfp_pack_create": (
         C.c_int,
         [C.c_int, C.c_int, c_int64_p, c_int64_p, c_double_pp, c_double_pp, c_double_pp, c_double_pp,
@@ -355,22 +357,31 @@ class Pack:
         """Loudest of ``S`` sky positions per frequency: ``fplus``, ``fcross`` host arrays ``(S, P)``. Returns / fills
         ``(fe_max, sky_index)``, ``(F,)`` float64 and int64. ``freqs`` / ``out`` as in :meth:`fp_sweep`; ``index_out``
         is a host int64 array when ``out`` is on the host, a device address when ``out`` is one."""
+        return self._skymax(load().fastfp_fe_skymax, None, freqs, fplus, fcross, out, index_out, stream)
+
+    def fe_skymax_residuals(self, freqs, fplus, fcross, out=None, index_out=None, stream: int = 0):
+        """:meth:`fe_skymax` for each realisation set by :meth:`set_residuals`: ``(fe_max, sky_index)`` of shape
+        ``(R, F)``. Always the fp64 kernel, whatever :attr:`path` says."""
+        return self._skymax(load().fastfp_fe_skymax_residuals, self.R, freqs, fplus, fcross, out, index_out, stream)
+
+    def _skymax(self, fn, rows, freqs, fplus, fcross, out, index_out, stream):
         fplus, fcross = as_f64(fplus), as_f64(fcross)
         if fplus.ndim != 2 or fplus.shape != fcross.shape or fplus.shape[1] != self.P:
             raise ValueError("fplus and fcross must both have shape (n_sky, n_pulsars)")
         S = fplus.shape[0]
-        freqs, out, F, ret, flags = self._stage(freqs, out)
+        freqs, out, F, ret, flags = self._stage(freqs, out, rows)
+        shape = (F,) if rows is None else (rows, F)
         iret = None
         if flags & OUT_ON_DEVICE:
             if index_out is None or isinstance(index_out, np.ndarray):
                 raise ValueError("out is a device address, so index_out must be one too")
         elif index_out is None:
-            index_out = iret = np.empty(F, dtype=np.int64)
-        elif not (isinstance(index_out, np.ndarray) and index_out.dtype == np.int64 and index_out.shape == (F,)
+            index_out = iret = np.empty(shape, dtype=np.int64)
+        elif not (isinstance(index_out, np.ndarray) and index_out.dtype == np.int64 and index_out.shape == shape
                   and index_out.flags.c_contiguous):
-            raise ValueError("index_out must be a contiguous int64 host array of shape (F,)")
-        check(load().fastfp_fe_skymax(self._h, _vp(freqs), F, _vp(fplus), _vp(fcross), S, _vp(out), _vp(index_out),
-                                      flags, C.c_void_p(stream)))
+            raise ValueError("index_out must be a contiguous int64 host array of shape " + ("(F,)" if rows is None else "(R, F)"))
+        check(fn(self._h, _vp(freqs), F, _vp(fplus), _vp(fcross), S, _vp(out), _vp(index_out), flags,
+                 C.c_void_p(stream)))
         return ret, iret
 
     def set_residuals(self, residuals, stream: int = 0) -> None:

@@ -585,6 +585,63 @@ int fastfp_fe_skymax(const fastfp_pack_t* pk, const double* freqs, int64_t F, co
   return FASTFP_OK;
 }
 
+// Sky-maximised Fe of each residual realisation (DESIGN.md section 5e): per frequency batch, the residual sweep writes
+// the inner products and fe_skymax_res_kernel reduces over the sky
+int fastfp_fe_skymax_residuals(const fastfp_pack_t* pk, const double* freqs, int64_t F, const double* fplus,
+                               const double* fcross, int64_t S, double* fe_max, int64_t* sky_index, int flags,
+                               void* stream) {
+  if (!pk || F < 0 || S < 0 || (F > 0 && (!freqs || !fe_max || !sky_index || (S > 0 && (!fplus || !fcross))))) {
+    set_error("fastfp_fe_skymax_residuals: null argument or negative size");
+    return FASTFP_ERR_INVALID;
+  }
+  if (pk->nmfp) {
+    set_error("fastfp_fe_skymax_residuals needs a plain-Fp pack (fastfp_pack_create)");
+    return FASTFP_ERR_INVALID;
+  }
+  if (pk->res_R == 0) {
+    set_error("fastfp_fe_skymax_residuals: no residual realisations set (fastfp_pack_set_residuals)");
+    return FASTFP_ERR_INVALID;
+  }
+  if (F == 0) return FASTFP_OK;
+  if (S == 0) { set_error("fastfp_fe_skymax_residuals needs at least one sky position"); return FASTFP_ERR_INVALID; }
+  const int P = pk->P;
+  const int64_t R = pk->res_R;
+  PackCall c(pk, stream);
+  const double* d_freqs;
+  double* d_max;
+  if (int rc = c.stage(freqs, F, fe_max, R * F, flags, &d_freqs, &d_max, &pk->d_out, &pk->out_cap)) return rc;
+  const int64_t FB = std::max<int64_t>(1024, std::min<int64_t>(F, kTermBudgetDoubles / ((2 * R + 3) * P)));
+  const int64_t fb0 = std::min(FB, F);
+  // the sky is split across CTAs only in a single-batch call: the per-chunk bests are merged into (R, F) columns
+  const FeSkyPlan plan = fe_skymax_res_plan(fb0, R, S, pk->num_sms, F <= FB);
+  // scratch: (s|r_k), (c|r_k) of one frequency batch in the residual terms buffer; in the Fe buffer (s|s), (s|c), (c|c)
+  // of the batch, the antenna patterns, the per-chunk bests of a split sky and the indices on their way to host memory
+  const int64_t n_mi = 3 * (int64_t)P * fb0, n_part = plan.nchunk > 1 ? plan.nchunk * R * fb0 : 0;
+  const int64_t n_idx = (flags & FASTFP_OUT_ON_DEVICE) ? 0 : R * F;
+  if (int rc = ensure(&pk->d_res_terms, &pk->res_terms_cap, 2 * R * P * fb0)) return rc;
+  if (int rc = ensure(&pk->d_inner, &pk->inner_cap, n_mi + 2 * S * P + 2 * n_part + n_idx)) return rc;
+  double* d_fp = pk->d_inner + n_mi;
+  double* d_fx = d_fp + S * P;
+  double* part_v = d_fx + S * P;
+  int64_t* part_i = reinterpret_cast<int64_t*>(part_v + n_part);
+  int64_t* d_idx = n_idx ? part_i + n_part : sky_index;
+  FFP_CUDA(cudaMemcpyAsync(d_fp, fplus, (size_t)S * P * 8, cudaMemcpyHostToDevice, c.st));
+  FFP_CUDA(cudaMemcpyAsync(d_fx, fcross, (size_t)S * P * 8, cudaMemcpyHostToDevice, c.st));
+  for (int64_t lo = 0; lo < F; lo += FB) {
+    const int64_t fb = std::min(FB, F - lo);
+    if (int rc = launch_fp_sweep_res(pk, d_freqs + lo, fb, pk->d_res_terms, c.st, pk->d_inner)) return rc;
+    if (int rc = launch_fe_skymax_res(pk->d_res_terms, pk->d_inner, P, R, fb, d_fp, d_fx, S, plan, part_v, part_i,
+                                      d_max + lo, d_idx + lo, F, c.st))
+      return rc;
+  }
+  if (!(flags & FASTFP_OUT_ON_DEVICE)) {
+    FFP_CUDA(cudaMemcpyAsync(fe_max, d_max, (size_t)(R * F) * 8, cudaMemcpyDeviceToHost, c.st));
+    FFP_CUDA(cudaMemcpyAsync(sky_index, d_idx, (size_t)(R * F) * 8, cudaMemcpyDeviceToHost, c.st));
+  }
+  FFP_CUDA(cudaStreamSynchronize(c.st));  // fplus / fcross were read from caller-owned host memory
+  return FASTFP_OK;
+}
+
 int fastfp_nmfp_sweep(const fastfp_pack_t* pk, const double* freqs, int64_t F,
                       const double* phiinv_var, int64_t D, double* out, int flags, void* stream) {
   if (!pk || F < 0 || D < 0 || ((F > 0 && D > 0) && (!freqs || !phiinv_var || !out))) {

@@ -227,7 +227,287 @@ __global__ void fe_skymax_merge_kernel(const double* __restrict__ part_v, const 
   idx_out[f] = bidx;
 }
 
-int launch_fe_sky_weights(const double* d_fplus, const double* d_fcross, int64_t n, double* d_w, cudaStream_t st) {
+// ---- sky maximum of a residual batch (DESIGN.md section 5e) ---------------------------------------------------
+// M(s, f) does not depend on the realisation and N_k(s, f) is linear in it: across realisations, N is the GEMM
+//   [(s|r_k), (c|r_k)]  (rows (k, f), K = pulsars)  x  [F+, Fx]  (columns (s, +/x))
+// on the fp64 MMA path, and M(s, f) is formed (fe_accumulate's FMAs, pulsar order) and factored (fe_solve's LU with
+// partial pivoting) once per (sky, frequency) and CTA, then applied to the N_k of every realisation the CTA holds.
+// A CTA owns kResRows rows (realisation, frequency) -- kt realisations x 64/kt frequencies, kt a power of two from 8
+// to 64 -- and one contiguous chunk of the sky, walked in passes of kResSC positions; its (s|r), (c|r) tile crosses
+// DRAM once when all pulsars fit one chunk of kResPC. Warp w holds row tiles 2(w&3), 2(w&3)+1 and column tiles
+// 4(w>>2) .. +3 (4 sky positions each) of a pass. The back substitution multiplies by the reciprocal of each pivot
+// instead of dividing, so values match fastfp_fe_skymax to rounding, not bit for bit.
+constexpr int kResRows = 64;                 // (realisation, frequency) rows per CTA: 8 MMA row tiles
+constexpr int kResSC = 32;                   // sky positions per pass: 8 MMA column tiles of 4 positions x {+, x}
+constexpr int kResPC = 48;                   // pulsars per shared-memory chunk (12 k-blocks)
+constexpr int kResKB = kResPC / 4;
+constexpr int kResThreads = 256;
+constexpr int kResWS = 2 * kResSC + 4;       // pulsar stride of the pattern tile: conflict-free B fragments
+constexpr int kResFac = 17;                  // doubles per factored M: 6 multipliers, 6 of U, 4 reciprocals, pivots
+constexpr size_t kResSmem = (size_t)(kResRows * kResPC * 2 + kResPC * kResWS + kResSC * 8 * kResFac) * sizeof(double);
+
+// D(8x8) += A(8x4) . B(4x8), fp64. Lane l holds A[l>>2][l&3], B[l&3][l>>2], D[l>>2][2*(l&3)+{0,1}].
+__device__ __forceinline__ void fe_dmma(double& d0, double& d1, double a, double b) {
+  asm("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
+      : "+d"(d0), "+d"(d1)
+      : "d"(a), "d"(b));
+}
+
+// fe_solve's elimination on M alone: o = [l10 l20 l30 l21 l31 l32 | u01 u02 u03 u12 u13 u23 | 1/u00 .. 1/u33 | pivots]
+__device__ __forceinline__ void fe_factor(const double (&U)[4][4], double* o) {
+  double M[4][4] = {{U[0][0], U[0][1], U[0][2], U[0][3]}, {U[0][1], U[1][1], U[1][2], U[1][3]},
+                    {U[0][2], U[1][2], U[2][2], U[2][3]}, {U[0][3], U[1][3], U[2][3], U[3][3]}};
+  int code = 0, li = 0;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    int piv = c;
+    double big = fabs(M[c][c]);
+#pragma unroll
+    for (int r = c + 1; r < 4; ++r) {
+      const double v = fabs(M[r][c]);
+      if (v > big) { big = v; piv = r; }
+    }
+#pragma unroll
+    for (int r = c + 1; r < 4; ++r) {
+      if (r == piv) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { const double t = M[c][j]; M[c][j] = M[r][j]; M[r][j] = t; }
+      }
+    }
+    code |= piv << (2 * c);
+#pragma unroll
+    for (int r = c + 1; r < 4; ++r) {
+      const double l = __ddiv_rn(M[r][c], M[c][c]);
+#pragma unroll
+      for (int j = c + 1; j < 4; ++j) M[r][j] = __fma_rn(-l, M[c][j], M[r][j]);
+      o[li++] = l;
+    }
+  }
+  o[6] = M[0][1]; o[7] = M[0][2]; o[8] = M[0][3]; o[9] = M[1][2]; o[10] = M[1][3]; o[11] = M[2][3];
+#pragma unroll
+  for (int r = 0; r < 4; ++r) o[12 + r] = __drcp_rn(M[r][r]);
+  o[16] = (double)code;
+}
+
+// 0.5 N^T M^-1 N with M factored by fe_factor: fe_solve's row swaps and updates of b, then back substitution
+__device__ __forceinline__ double fe_apply(const double (&N)[4], const double* o) {
+  double b[4] = {N[0], N[1], N[2], N[3]};
+  const int code = (int)o[16];
+  int li = 0;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const int piv = (code >> (2 * c)) & 3;
+#pragma unroll
+    for (int r = c + 1; r < 4; ++r) {
+      const bool sw = r == piv;
+      const double t = sw ? b[r] : b[c];
+      b[r] = sw ? b[c] : b[r];
+      b[c] = t;
+    }
+#pragma unroll
+    for (int r = c + 1; r < 4; ++r) b[r] = __fma_rn(-o[li++], b[c], b[r]);
+  }
+  double x[4];
+  x[3] = __dmul_rn(b[3], o[15]);
+  x[2] = __dmul_rn(__fma_rn(-o[11], x[3], b[2]), o[14]);
+  x[1] = __dmul_rn(__fma_rn(-o[10], x[3], __fma_rn(-o[9], x[2], b[1])), o[13]);
+  x[0] = __dmul_rn(__fma_rn(-o[8], x[3], __fma_rn(-o[7], x[2], __fma_rn(-o[6], x[1], b[0]))), o[12]);
+  const double d = __fma_rn(N[0], x[0], __dmul_rn(N[1], x[1]));
+  return __dmul_rn(0.5, __fma_rn(N[3], x[3], __fma_rn(N[2], x[2], d)));
+}
+
+__global__ void __launch_bounds__(kResThreads, 2)
+    fe_skymax_res_kernel(const double* __restrict__ X, const double* __restrict__ Mi, int P, int R, int ktlog, int64_t F,
+                         const double* __restrict__ fplus, const double* __restrict__ fcross, int64_t S, int64_t chunk,
+                         double* __restrict__ best_out, int64_t* __restrict__ idx_out, int64_t ld, int64_t zstride) {
+  extern __shared__ double sh[];
+  double* sA = sh;                                   // [8 row tiles][kResKB][s|c][32]    A fragments
+  double* sW = sA + kResRows * kResPC * 2;           // [kResPC][kResWS]: (F+, Fx) of each sky position of the pass
+  double* sFac = sW + kResPC * kResWS;               // [64/kt frequencies][kResSC][kResFac]
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int wr = warp & 3, wc = warp >> 2;
+  const int kt = 1 << ktlog, ft = kResRows >> ktlog;
+  const int64_t f0 = (int64_t)blockIdx.x * ft;
+  const int k0 = blockIdx.y * kt;
+  const int64_t s_begin = (int64_t)blockIdx.z * chunk;
+  const int64_t s_end = min(S, s_begin + chunk);
+  const bool resident = P <= kResPC;
+  const double nan = __longlong_as_double(0x7ff8000000000000LL);
+  // the M-stage thread of (frequency fl, sky position sl of the pass)
+  const int m_fl = tid / kResSC, m_sl = tid % kResSC;
+  const int64_t m_f = f0 + m_fl;
+  const bool m_on = m_fl < ft && m_f < F;
+  double best[2] = {nan, nan};
+  int64_t bidx[2] = {-1, -1};
+  for (int64_t s0 = s_begin; s0 < s_end; s0 += kResSC) {
+    const int ns = s_end - s0 < kResSC ? (int)(s_end - s0) : kResSC;
+    double acc[2][4][2][2] = {};
+    for (int p0 = 0; p0 < P; p0 += kResPC) {
+      const int pc = min(kResPC, P - p0);
+      __syncthreads();  // the previous pass or chunk is done with the tiles
+      if (!resident || s0 == s_begin) {
+        // A fragments, walked in the order of X ([f][p][k][s|c]); rows and pulsars outside the problem are zero
+        for (int i = tid; i < kResRows * kResPC * 2; i += kResThreads) {
+          const int sc = i & 1, kl = (i >> 1) & (kt - 1), rest = i >> (1 + ktlog);
+          const int pl = rest % kResPC, fl = rest / kResPC;
+          const int row = (fl << ktlog) | kl, k = k0 + kl;
+          const int64_t f = f0 + fl;
+          const double v = (pl < pc && k < R && f < F) ? X[((f * P + p0 + pl) * R + k) * 2 + sc] : 0.0;
+          sA[(((row >> 3) * kResKB + (pl >> 2)) * 2 + sc) * 32 + ((row & 7) << 2) + (pl & 3)] = v;
+        }
+      }
+      for (int i = tid; i < kResSC * kResPC; i += kResThreads) {
+        const int pl = i % kResPC, sl = i / kResPC;
+        const bool in = pl < pc && sl < ns;
+        const size_t g = (size_t)(s0 + sl) * P + p0 + pl;
+        sW[pl * kResWS + 2 * sl] = in ? fplus[g] : 0.0;
+        sW[pl * kResWS + 2 * sl + 1] = in ? fcross[g] : 0.0;
+      }
+      __syncthreads();
+      if (m_on && m_sl < ns) {
+        // M(s, f): fe_accumulate's M updates, pulsars in order. Between pulsar chunks the partial sums wait in this
+        // thread's factor slot, so they hold no registers during the MMAs.
+        double* slot = sFac + (m_fl * kResSC + m_sl) * kResFac;
+        double Mu[4][4] = {};
+        if (p0 > 0) {
+          Mu[0][0] = slot[0]; Mu[0][1] = slot[1]; Mu[0][2] = slot[2]; Mu[0][3] = slot[3]; Mu[1][1] = slot[4];
+          Mu[1][2] = slot[5]; Mu[1][3] = slot[6]; Mu[2][2] = slot[7]; Mu[2][3] = slot[8]; Mu[3][3] = slot[9];
+        }
+        for (int pl = 0; pl < pc; ++pl) {
+          const double2 w = *reinterpret_cast<const double2*>(sW + pl * kResWS + 2 * m_sl);
+          const double* q = Mi + ((size_t)m_f * P + p0 + pl) * 3;
+          const double ss = __ldg(q), sc = __ldg(q + 1), cc = __ldg(q + 2);
+          const double fp = w.x, fx = w.y, pp = __dmul_rn(fp, fp), px = __dmul_rn(fp, fx), xx = __dmul_rn(fx, fx);
+          Mu[0][0] = __fma_rn(pp, ss, Mu[0][0]); Mu[0][1] = __fma_rn(pp, sc, Mu[0][1]);
+          Mu[1][1] = __fma_rn(pp, cc, Mu[1][1]);
+          Mu[0][2] = __fma_rn(px, ss, Mu[0][2]); Mu[0][3] = __fma_rn(px, sc, Mu[0][3]);
+          Mu[1][2] = __fma_rn(px, sc, Mu[1][2]); Mu[1][3] = __fma_rn(px, cc, Mu[1][3]);
+          Mu[2][2] = __fma_rn(xx, ss, Mu[2][2]); Mu[2][3] = __fma_rn(xx, sc, Mu[2][3]);
+          Mu[3][3] = __fma_rn(xx, cc, Mu[3][3]);
+        }
+        if (p0 + kResPC < P) {
+          slot[0] = Mu[0][0]; slot[1] = Mu[0][1]; slot[2] = Mu[0][2]; slot[3] = Mu[0][3]; slot[4] = Mu[1][1];
+          slot[5] = Mu[1][2]; slot[6] = Mu[1][3]; slot[7] = Mu[2][2]; slot[8] = Mu[2][3]; slot[9] = Mu[3][3];
+        } else {
+          fe_factor(Mu, slot);
+        }
+      }
+      // N: 2 row tiles x 4 column tiles x {s, c} MMAs per k-block
+      const double* a_p = sA + (2 * wr) * kResKB * 64 + lane;
+      const double* b_p = sW + (lane & 3) * kResWS + (4 * wc * 4 + (lane >> 3)) * 2 + ((lane >> 2) & 1);
+      const int nkb = (pc + 3) >> 2;
+#pragma unroll 2
+      for (int kb = 0; kb < nkb; ++kb) {
+        double a[2][2], b[4];
+#pragma unroll
+        for (int rt = 0; rt < 2; ++rt)
+#pragma unroll
+          for (int sc = 0; sc < 2; ++sc) a[rt][sc] = a_p[((rt * kResKB + kb) * 2 + sc) * 32];
+#pragma unroll
+        for (int ct = 0; ct < 4; ++ct) b[ct] = b_p[4 * kb * kResWS + ct * 8];
+#pragma unroll
+        for (int rt = 0; rt < 2; ++rt)
+#pragma unroll
+          for (int ct = 0; ct < 4; ++ct)
+#pragma unroll
+            for (int sc = 0; sc < 2; ++sc) fe_dmma(acc[rt][ct][sc][0], acc[rt][ct][sc][1], a[rt][sc], b[ct]);
+      }
+    }
+    __syncthreads();  // the factors of the pass are published
+#pragma unroll
+    for (int rt = 0; rt < 2; ++rt) {
+      const int row = 8 * (2 * wr + rt) + (lane >> 2);
+      const int fl = row >> ktlog;
+#pragma unroll
+      for (int ct = 0; ct < 4; ++ct) {
+        const int sl = 4 * (4 * wc + ct) + (lane & 3);
+        if (sl >= ns) continue;
+        // this lane's N: [F+ (s|r), F+ (c|r), Fx (s|r), Fx (c|r)]
+        const double N[4] = {acc[rt][ct][0][0], acc[rt][ct][1][0], acc[rt][ct][0][1], acc[rt][ct][1][1]};
+        const double v = fe_apply(N, sFac + (fl * kResSC + sl) * kResFac);
+        if (fe_better(v, s0 + sl, best[rt], bidx[rt])) { best[rt] = v; bidx[rt] = s0 + sl; }
+      }
+    }
+  }
+  // merge the 4 lanes of a row, then the two warps of a row tile pair
+#pragma unroll
+  for (int rt = 0; rt < 2; ++rt)
+#pragma unroll
+    for (int m = 1; m <= 2; m <<= 1) {
+      const double v = __shfl_xor_sync(0xffffffffu, best[rt], m);
+      const int64_t i = __shfl_xor_sync(0xffffffffu, bidx[rt], m);
+      if (fe_better(v, i, best[rt], bidx[rt])) { best[rt] = v; bidx[rt] = i; }
+    }
+  __syncthreads();
+  double* sv = sh;
+  int64_t* si = reinterpret_cast<int64_t*>(sh + kResRows);
+  if (wc == 1 && (lane & 3) == 0)
+#pragma unroll
+    for (int rt = 0; rt < 2; ++rt) {
+      const int row = 8 * (2 * wr + rt) + (lane >> 2);
+      sv[row] = best[rt];
+      si[row] = bidx[rt];
+    }
+  __syncthreads();
+  if (wc == 0 && (lane & 3) == 0)
+#pragma unroll
+    for (int rt = 0; rt < 2; ++rt) {
+      const int row = 8 * (2 * wr + rt) + (lane >> 2);
+      if (fe_better(sv[row], si[row], best[rt], bidx[rt])) { best[rt] = sv[row]; bidx[rt] = si[row]; }
+      const int k = k0 + (row & (kt - 1));
+      const int64_t f = f0 + (row >> ktlog);
+      if (k < R && f < F) {
+        const size_t o = (size_t)blockIdx.z * zstride + (size_t)k * ld + f;
+        best_out[o] = best[rt];
+        idx_out[o] = bidx[rt];
+      }
+    }
+}
+
+static int res_ktlog(int64_t R) {
+  int l = 3;
+  while (l < 6 && ((int64_t)1 << l) < R) ++l;
+  return l;
+}
+
+// Split of the sky axis, as fe_skymax_plan: about four rounds of the GPU at two CTAs per SM, in whole passes; one
+// chunk unless may_split
+FeSkyPlan fe_skymax_res_plan(int64_t F, int64_t R, int64_t S, int num_sms, bool may_split) {
+  const int ktlog = res_ktlog(R);
+  const int64_t ft = kResRows >> ktlog;
+  const int64_t tiles = ((F + ft - 1) / ft) * ((R + (1 << ktlog) - 1) >> ktlog);
+  const int64_t passes = (S + kResSC - 1) / kResSC;
+  const int64_t want = may_split ? std::max<int64_t>(1, (4 * 2 * (int64_t)std::max(num_sms, 1) + tiles - 1) / tiles) : 1;
+  const int64_t per = (passes + std::min(want, passes) - 1) / std::min(want, passes);
+  FeSkyPlan pl;
+  pl.chunk = per * kResSC;
+  pl.nchunk = (passes + per - 1) / per;
+  return pl;
+}
+
+int launch_fe_skymax_res(const double* d_x, const double* d_mi, int P, int64_t R, int64_t F, const double* d_fplus,
+                         const double* d_fcross, int64_t S, const FeSkyPlan& pl, double* d_part_v, int64_t* d_part_i,
+                         double* d_best, int64_t* d_idx, int64_t ld, cudaStream_t st) {
+  FFP_CUDA(cudaFuncSetAttribute(fe_skymax_res_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kResSmem));
+  const int ktlog = res_ktlog(R);
+  const bool split = pl.nchunk > 1;
+  dim3 grid((unsigned)((F + (kResRows >> ktlog) - 1) / (kResRows >> ktlog)), (unsigned)((R + (1 << ktlog) - 1) >> ktlog),
+            (unsigned)pl.nchunk);
+  fe_skymax_res_kernel<<<grid, kResThreads, kResSmem, st>>>(d_x, d_mi, P, (int)R, ktlog, F, d_fplus, d_fcross, S,
+                                                            pl.chunk, split ? d_part_v : d_best, split ? d_part_i : d_idx,
+                                                            split ? F : ld, split ? R * F : 0);
+  g_launches += 1;
+  FFP_CUDA(cudaGetLastError());
+  if (split) {  // the per-chunk bests of every (realisation, frequency) column, merged in chunk order
+    fe_skymax_merge_kernel<<<(unsigned)((R * F + 127) / 128), 128, 0, st>>>(d_part_v, d_part_i, pl.nchunk, R * F,
+                                                                             d_best, d_idx);
+    g_launches += 1;
+    FFP_CUDA(cudaGetLastError());
+  }
+  return 0;
+}
+
+int launch_fe_sky_weights(const double* d_fplus,const double* d_fcross, int64_t n, double* d_w, cudaStream_t st) {
   if (n == 0) return 0;
   fe_sky_weights_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_fplus, d_fcross, n, d_w);
   g_launches += 1;

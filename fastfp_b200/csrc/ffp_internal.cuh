@@ -257,8 +257,9 @@ int launch_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, double
                  const NmfpOut* nm = nullptr, double* d_inner = nullptr);
 int launch_reduce_terms(const double* d_terms, int P, int64_t F, double* d_out, cudaStream_t st);
 // residual batches: the sweep over the pack's residual packets (terms [R][P][F]) and the pulsar sum of each row
-// into out[k * ld + f]
-int launch_fp_sweep_res(const fastfp_pack* pk, const double* d_freqs, int64_t F, double* d_terms, cudaStream_t st);
+// into out[k * ld + f]; with d_minner the sweep writes the Fe inner products instead (fp_sweep.cu)
+int launch_fp_sweep_res(const fastfp_pack* pk, const double* d_freqs, int64_t F, double* d_terms, cudaStream_t st,
+                        double* d_minner = nullptr);
 int launch_reduce_terms_rows(const double* d_terms, int R, int P, int64_t F, double* d_out, int64_t ld,
                              cudaStream_t st);
 // fp_sweep_i8.cu
@@ -280,6 +281,13 @@ FeSkyPlan fe_skymax_plan(int64_t F, int64_t S, int num_sms);
 int launch_fe_sky_weights(const double* d_fplus, const double* d_fcross, int64_t n, double* d_w, cudaStream_t st);
 int launch_fe_skymax(const double* d_inner, int P, int64_t F, const double* d_w, int64_t S, const FeSkyPlan& pl,
                      double* d_part_v, int64_t* d_part_i, double* d_best, int64_t* d_idx, cudaStream_t st);
+// sky maximum of a residual batch (DESIGN.md section 5e): d_x = (s|r_k), (c|r_k) as [F][P][R][2] and d_mi = (s|s),
+// (s|c), (c|c) as [F][P][3] from launch_fp_sweep_res; d_fplus / d_fcross (S, P). Writes (R, F) with row stride ld; a
+// plan with nchunk > 1 needs ld == F and the (nchunk, R, F) scratch d_part_v / d_part_i.
+FeSkyPlan fe_skymax_res_plan(int64_t F, int64_t R, int64_t S, int num_sms, bool may_split);
+int launch_fe_skymax_res(const double* d_x, const double* d_mi, int P, int64_t R, int64_t F, const double* d_fplus,
+                         const double* d_fcross, int64_t S, const FeSkyPlan& pl, double* d_part_v, int64_t* d_part_i,
+                         double* d_best, int64_t* d_idx, int64_t ld, cudaStream_t st);
 bool sweep_config(int m, KernelCfg* cfg);
 int sweep_max_slab_doubles();
 // xcy.cu

@@ -85,14 +85,17 @@ int launch_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, double
 }
 
 // The residual batch (DESIGN.md section 5d): the fp64 kernel on the pack's residual packets, whose G tiles carry
-// the realisations' w_k as extra rows; terms is [R][P][F].
-int launch_fp_sweep_res(const fastfp_pack* pk, const double* d_freqs, int64_t F, double* d_terms, cudaStream_t st) {
+// the realisations' w_k as extra rows; terms is [R][P][F]. With d_minner (DESIGN.md section 5e) the kernel writes inner
+// products instead: d_terms gets (s|r_k), (c|r_k) as [F][P][R][2] and d_minner (s|s), (s|c), (c|c) as [F][P][3].
+int launch_fp_sweep_res(const fastfp_pack* pk, const double* d_freqs, int64_t F, double* d_terms, cudaStream_t st,
+                        double* d_minner) {
   SweepArgs a{};
   a.packets = pk->d_res_packets;
   a.meta = pk->d_res_meta;
   a.freqs = d_freqs;
   a.F = F;
   a.terms = d_terms;
+  a.inner = d_minner;
   a.slab = pk->d_slab;
   a.counter = pk->d_counter;
   a.nres = (int)pk->res_R;

@@ -54,7 +54,9 @@ struct SweepArgs {
   double* A;              // nmfp: [P][ceil(F/32)][5][32]
   int mvmax;
   const unsigned char* done_mask;  // block-N packs: per chunk, which of the 8 epoch slots end there
-  int nres;   // residual batches: realisations, in rows roundup8(m) .. roundup8(m)+nres-1 of G; terms is [nres][npsr][F]
+  // residual batches: realisations, in rows roundup8(m) .. roundup8(m)+nres-1 of G; terms is [nres][npsr][F], or with
+  // inner set (Fe over residual batches) terms is [F][npsr][nres][2] ((s|r_k), (c|r_k)) and inner is [F][npsr][3]
+  int nres;
   int npsr;
 #ifdef FFP_DEBUG_SWITCHES
   int dbg;  // profiling builds only (tools/dbg_split.sh): bit 0 producers' math off, 1 MMAs off, 2 level-2 flush off
@@ -507,6 +509,12 @@ __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>&
         redB[tid * 3 + 0] = a[0] - b[0];
         redB[tid * 3 + 1] = a[1] - b[1];
         redB[tid * 3 + 2] = a[2] - b[2];
+        if (ar.inner) {  // inner-product output: (s|s), (s|c), (c|c) as [F][P][3], NaN at f <= 0 (Fe is even in f)
+          double* o = ar.inner + ((size_t)fidx * ar.npsr + p) * 3;
+          const bool fpos = sm.fq[tid] > 0.0;
+#pragma unroll
+          for (int k = 0; k < 3; ++k) o[k] = fpos ? a[k] - b[k] : __longlong_as_double(0x7ff8000000000000LL);
+        }
       } else {
         // M = [[ss, sc],[sc, cc]], N = [(s|r), (c|r)]
         double val = term_2x2(a[0] - b[0], a[1] - b[1], a[2] - b[2], a[3], a[4]);
@@ -537,6 +545,12 @@ __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>&
         for (int r = 0; r < NMBW; ++r) {
           const int k = 8 * (wm * NMBW + r) + (lane >> 2) - r0;
           if (k < 0 || k >= ar.nres) continue;
+          if (ar.inner) {  // inner-product output: (s|r_k), (c|r_k) as [F][P][R][2]
+            const double nan = __longlong_as_double(0x7ff8000000000000LL);
+            *reinterpret_cast<double2*>(ar.terms + (((size_t)f * ar.npsr + p) * ar.nres + k) * 2) =
+                fpos ? make_double2(acc[r][q][0], acc[r][q][1]) : make_double2(nan, nan);
+            continue;
+          }
           double val = term_2x2(m00, m01, m11, acc[r][q][0], acc[r][q][1]);
           if (!fpos) val = __longlong_as_double(0x7ff8000000000000LL);
           ar.terms[((size_t)k * ar.npsr + p) * ar.F + f] = val;

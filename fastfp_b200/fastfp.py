@@ -257,29 +257,8 @@ class FastFp(_PackCache):
         at m = 72); ``R`` is split into passes of :func:`batch_pass_rows` rows, the split with the least modelled
         sweep cost (measured per-row costs of the kernel configurations). The pass size selects the kernel configuration, so values can differ in the last bits
         between different ``R``; within one ``R`` every row is computed alike wherever it sits."""
-        res = [_cabi.as_f64(r) for r in residuals]
-        if len(res) != len(self.toas):
-            raise ValueError(f"residuals must be a list of {len(self.toas)} arrays (one per pulsar)")
-        R = res[0].shape[0] if res[0].ndim == 2 else -1
-        for p, r in enumerate(res):
-            if r.shape != (R, self.toas[p].shape[0]):
-                raise ValueError(f"residuals[{p}] must have shape (R, {self.toas[p].shape[0]}) with the same R >= 1 for "
-                                 f"every pulsar; got {r.shape}")
-        if R < 1:
-            raise ValueError("residuals must hold at least one realisation")
+        R, passes = self._residual_passes(residuals)
         lists = (Nvecs, Ts, sigmas)
-        res_key = _fingerprint([res])
-
-        def passes(pack, stream=0):
-            rows = batch_pass_rows(R, pack.m)
-            for lo in range(0, R, rows):
-                hi = min(R, lo + rows)
-                key = (res_key, lo, hi)
-                if self._res_pack is not pack or self._res_key != key:
-                    self._res_pack, self._res_key = None, None
-                    pack.set_residuals([r[lo:hi] for r in res], stream=stream)
-                    self._res_pack, self._res_key = pack, key
-                yield lo, hi
 
         if _is_cuda_tensor(fgw):
             import torch
@@ -303,6 +282,35 @@ class FastFp(_PackCache):
             return out
 
         return self._run_verified(lists, run, asynchronous=False).reshape((R,) + f.shape)
+
+    def _residual_passes(self, residuals):
+        """Checks the shapes of ``residuals`` (a list of ``P`` arrays ``(R, n_p)``) and returns ``(R, passes)``:
+        ``passes(pack, stream=0)`` yields the row ranges ``(lo, hi)`` of :func:`batch_pass_rows` passes with each
+        pass's realisations set on ``pack``, uploaded again only when the pack or any byte of them changed."""
+        res = [_cabi.as_f64(r) for r in residuals]
+        if len(res) != len(self.toas):
+            raise ValueError(f"residuals must be a list of {len(self.toas)} arrays (one per pulsar)")
+        R = res[0].shape[0] if res[0].ndim == 2 else -1
+        for p, r in enumerate(res):
+            if r.shape != (R, self.toas[p].shape[0]):
+                raise ValueError(f"residuals[{p}] must have shape (R, {self.toas[p].shape[0]}) with the same R >= 1 for "
+                                 f"every pulsar; got {r.shape}")
+        if R < 1:
+            raise ValueError("residuals must hold at least one realisation")
+        res_key = _fingerprint([res])
+
+        def passes(pack, stream=0):
+            rows = batch_pass_rows(R, pack.m)
+            for lo in range(0, R, rows):
+                hi = min(R, lo + rows)
+                key = (res_key, lo, hi)
+                if self._res_pack is not pack or self._res_key != key:
+                    self._res_pack, self._res_key = None, None
+                    pack.set_residuals([r[lo:hi] for r in res], stream=stream)
+                    self._res_pack, self._res_key = pack, key
+                yield lo, hi
+
+        return R, passes
 
     _res_pack = None
     _res_key = None

@@ -77,14 +77,7 @@ class FastFe(FastFp):
         ``fgw``'s shape for an array, CUDA tensors on its device (enqueued on torch's current stream) for a float64
         CUDA tensor. Each value equals the corresponding entry of :meth:`calculate_Fe`'s map bit for bit; NaN loses,
         ties go to the lowest index, and a frequency with no finite value gives ``(nan, -1)``."""
-        try:
-            th, ph = np.broadcast_arrays(np.atleast_1d(np.asarray(gwtheta, dtype=np.float64)),
-                                         np.atleast_1d(np.asarray(gwphi, dtype=np.float64)))
-        except ValueError:
-            raise ValueError("gwtheta and gwphi must broadcast to one shape (S,)") from None
-        if th.ndim != 1:
-            raise ValueError("gwtheta and gwphi must broadcast to one shape (S,)")
-        fplus, fcross = antenna_pattern(self.pos, th, ph)  # (S, P)
+        fplus, fcross = self._sky_grid(gwtheta, gwphi)
         lists = (Nvecs, Ts, sigmas)
         if _is_cuda_tensor(fgw):
             import torch
@@ -106,3 +99,55 @@ class FastFe(FastFp):
         if f.ndim == 0:
             return float(best[0]), int(idx[0])
         return best.reshape(f.shape), idx.reshape(f.shape)
+
+    def calculate_Fe_skymax_batch(self, fgw, gwtheta, gwphi, Nvecs, Ts, sigmas, residuals):
+        """:meth:`calculate_Fe_skymax` for each of ``R`` realisations of the residuals, with the pulsars, noise model
+        and basis of ``Nvecs, Ts, sigmas``: the scan of simulated noise that calibrates an all-sky search's false-alarm
+        threshold (the maximum over correlated sky positions has no closed-form distribution), or of injected signals
+        for its detection probability. ``residuals`` is a list of ``P`` arrays ``(R, n_p)`` as for
+        :meth:`calculate_Fp_batch`, validated, cached and split into passes the same way. Returns ``(fe_max,
+        sky_index)``: ``(R,)`` for a scalar ``fgw``, ``(R, *fgw.shape)`` for an array, CUDA tensors on torch's current
+        stream for a float64 CUDA tensor. Row ``k`` is the sky maximum of Fe with residuals ``residuals[p][k]``, under
+        the same rule (NaN loses, ties go to the lowest index, ``(nan, -1)`` where no position is finite). Values meet
+        the parity bar of :meth:`calculate_Fe_skymax` but are not bit-identical to it (``fastfp_fe_skymax_residuals``,
+        DESIGN.md section 5e). One sky position is a targeted search at a known position."""
+        fplus, fcross = self._sky_grid(gwtheta, gwphi)
+        R, passes = self._residual_passes(residuals)
+        lists = (Nvecs, Ts, sigmas)
+        if _is_cuda_tensor(fgw):
+            import torch
+
+            f, stream = self._device_freqs(fgw)
+            best = torch.empty((R, f.shape[0]), dtype=torch.float64, device=f.device)
+            idx = torch.empty((R, f.shape[0]), dtype=torch.int64, device=f.device)
+
+            def run(pack):
+                for lo, _ in passes(pack, stream):
+                    pack.fe_skymax_residuals((f.data_ptr(), f.shape[0]), fplus, fcross, out=best[lo].data_ptr(),
+                                             index_out=idx[lo].data_ptr(), stream=stream)
+                return best, idx
+
+            best, idx = self._run_verified(lists, run, asynchronous=True)
+            return best.reshape((R,) + tuple(fgw.shape)), idx.reshape((R,) + tuple(fgw.shape))
+        f = np.asarray(fgw, dtype=np.float64)
+        fl = f.reshape(-1)
+
+        def run(pack):
+            best, idx = np.empty((R, fl.shape[0])), np.empty((R, fl.shape[0]), dtype=np.int64)
+            for lo, hi in passes(pack):
+                pack.fe_skymax_residuals(fl, fplus, fcross, out=best[lo:hi], index_out=idx[lo:hi])
+            return best, idx
+
+        best, idx = self._run_verified(lists, run, asynchronous=False)
+        return best.reshape((R,) + f.shape), idx.reshape((R,) + f.shape)
+
+    def _sky_grid(self, gwtheta, gwphi):
+        """Antenna patterns ``(F+, Fx)``, each ``(S, P)``, of the sky grid ``gwtheta``, ``gwphi`` broadcast to ``(S,)``."""
+        try:
+            th, ph = np.broadcast_arrays(np.atleast_1d(np.asarray(gwtheta, dtype=np.float64)),
+                                         np.atleast_1d(np.asarray(gwphi, dtype=np.float64)))
+        except ValueError:
+            raise ValueError("gwtheta and gwphi must broadcast to one shape (S,)") from None
+        if th.ndim != 1:
+            raise ValueError("gwtheta and gwphi must broadcast to one shape (S,)")
+        return antenna_pattern(self.pos, th, ph)

@@ -146,6 +146,27 @@ int fastfp_pack_set_residuals(fastfp_pack_t* pack, int64_t R, const double* cons
 int fastfp_fp_sweep_residuals(const fastfp_pack_t* pack, const double* freqs, int64_t F, double* out, int flags,
                               void* stream);
 
+/* fastfp_fe_skymax_residuals: the sky-maximised Fe of fastfp_fe_skymax for each realisation set by
+ *   fastfp_pack_set_residuals: fe_max[k*F + f] = max_s Fe_k(s, f), sky_index[k*F + f] = the s that attains it
+ *   (fe_max, sky_index: (R, F) row-major), with the reduction rule of fastfp_fe_skymax (NaN loses, ties go to the
+ *   lowest index, an all-NaN column gives NaN and -1). The false-alarm threshold of an all-sky search has no closed
+ *   form; this is the scan of simulated realisations that calibrates it. The values meet the parity bar of
+ *   fastfp_fe_skymax but are not bit-identical to it: (s|r_k), (c|r_k) come from the sweep's MMA, N_k from an MMA over
+ *   the pulsars, and the 4x4 solve multiplies by reciprocal pivots (DESIGN.md section 5e). It always runs the fp64
+ *   kernel, whatever fastfp_pack_path says. fplus, fcross: host arrays (S, P) row-major. flags as for fastfp_fp_sweep;
+ *   FASTFP_OUT_ON_DEVICE covers both outputs. Returns FASTFP_ERR_INVALID for a NULL argument, a negative size, an nmfp
+ *   pack, a pack with no realisations set (block-N packs cannot hold them), or S == 0 with F > 0; F == 0 returns
+ *   FASTFP_OK and writes nothing.
+ *   Device scratch, grown on demand and kept until fastfp_pack_destroy: the realisations' inner products of one
+ *   frequency batch, 2 R P F_batch doubles in the residual terms buffer (kept until the realisations are replaced or
+ *   released), and in the pack's Fe scratch 3 P F_batch + 2 S P doubles, plus R F for host outputs and, when the sky is
+ *   split across CTAs (a single batch of few frequencies), 2 R F per sky chunk; F_batch = max(1024, min(F, 2^27 /
+ *   ((2R + 3) P))). About 1.1 GB at R = 248, P = 45, F = 10^4, S = 3072. R F doubles for host outputs live in the
+ *   pack's output buffer as for fastfp_fp_sweep_residuals. */
+int fastfp_fe_skymax_residuals(const fastfp_pack_t* pack, const double* freqs, int64_t F, const double* fplus,
+                               const double* fcross, int64_t S, double* fe_max, int64_t* sky_index, int flags,
+                               void* stream);
+
 /* ---- noise-marginalised Fp -----------------------------------------------------------
  * fastfp_nmfp_pack_create: NMFP.__init__ (fastfp/nmfp.py:45-51) plus the (TNTs, Nvecs, Ts)
  * of get_mats_nmfp (fastfp/utils.py:97-101). Sigma_d = TNT + diag(phiinv_d) is formed per
