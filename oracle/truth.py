@@ -87,17 +87,74 @@ def _store(out, p, cols, **vals):
         out[k][p, cols] = v
 
 
-def terms_truth(inner):
-    """``(terms (P,F) longdouble, cond (P,F) float64)`` of :func:`fp_sweep_truth` from :func:`sweep_inner_truth`."""
+def _solve_2x2(inner):
     Mss, Msc, Mcc, Ns, Nc = (inner[k] for k in ("Mss", "Msc", "Mcc", "Ns", "Nc"))
     det = Mss * Mcc - Msc * Msc
-    x0 = (Mcc * Ns - Msc * Nc) / det
-    x1 = (Mss * Nc - Msc * Ns) / det
-    terms = LD(0.5) * (Ns * x0 + Nc * x1)
-    A0, A1, B00, B01, B11 = (inner[k] for k in ("A0", "A1", "B00", "B01", "B11"))
+    return (Mcc * Ns - Msc * Nc) / det, (Mss * Nc - Msc * Ns) / det
+
+
+def _first_order(x0, x1, A0, A1, B00, B01, B11):
+    """``|x|^T A + 0.5 |x|^T B |x|``: the first-order change of ``0.5 N^T M^-1 N`` for changes of ``N`` bounded by
+    ``A`` and of ``M`` by ``B``"""
     ax0, ax1 = np.abs(x0), np.abs(x1)
-    c = ax0 * A0 + ax1 * A1 + LD(0.5) * (ax0 * ax0 * B00 + 2 * ax0 * ax1 * B01 + ax1 * ax1 * B11)
+    return ax0 * A0 + ax1 * A1 + LD(0.5) * (ax0 * ax0 * B00 + 2 * ax0 * ax1 * B01 + ax1 * ax1 * B11)
+
+
+def terms_truth(inner):
+    """``(terms (P,F) longdouble, cond (P,F) float64)`` of :func:`fp_sweep_truth` from :func:`sweep_inner_truth`."""
+    x0, x1 = _solve_2x2(inner)
+    terms = LD(0.5) * (inner["Ns"] * x0 + inner["Nc"] * x1)
+    c = _first_order(x0, x1, *(inner[k] for k in ("A0", "A1", "B00", "B01", "B11")))
     return terms, c.astype(np.float64)
+
+
+def _bwd_ld(L, B):
+    """Solve L^T X = B (L lower triangular), longdouble, B: (m, k)."""
+    m = L.shape[0]
+    X = np.array(B, dtype=LD)
+    for j in range(m - 1, -1, -1):
+        X[j] = (X[j] - L[j + 1 :, j] @ X[j + 1 :]) / L[j, j]
+    return X
+
+
+def sigma_cond_truth(freqs, toas, residuals, Nvecs, Ts, sigmas, chunk=128):
+    """Conditioning of the per-pulsar terms of :func:`fp_sweep_truth` with respect to ``Sigma`` itself: ``(P, F)``
+    float64.
+
+    :func:`fp_sweep_truth`'s ``cond`` charges the rounding committed in the inner products for an exact ``Sigma``
+    solve. A float64 Cholesky of ``Sigma = L L^T`` is instead the exact factor of ``Sigma + dSigma`` with
+    ``|dSigma| <= gamma_(m+1) |L| |L^T|`` elementwise (Higham, *Accuracy and Stability of Numerical Algorithms*, Thm
+    10.3), and a badly conditioned ``Sigma`` (a loud, steep red process leaves ``Sigma ~ T^T N^-1 T``) turns that into
+    errors ``cond`` does not see. To first order ``d(x|y) = w_x^T dSigma w_y`` with ``w_x = Sigma^-1 T^T N^-1 x``, so
+    ``|d(x|y)| <= gamma * v_x^T v_y`` with ``v_x = |L^T| |w_x|``; these bounds go through the 2x2 solve as in ``cond``.
+    Returned in units of the rounding factor, like ``cond``."""
+    freqs = np.atleast_1d(np.asarray(freqs, dtype=np.float64))
+    F, P = freqs.shape[0], len(toas)
+    out = np.zeros((P, F))
+    for p in range(P):
+        toa = np.asarray(toas[p], dtype=np.float64)
+        ninv = LD(1) / np.asarray(Nvecs[p], dtype=LD)
+        T = np.asarray(Ts[p], dtype=LD)
+        r = np.asarray(residuals[p], dtype=LD)
+        L = _chol_ld(sigmas[p])
+        aLt = np.abs(L).T
+        G = _fwd_ld(L, (T * ninv[:, None]).T)  # (m, n): L^-1 T^T N^-1
+        ur = G @ r
+        vr = aLt @ np.abs(_bwd_ld(L, ur[:, None])[:, 0])
+        rn = r * ninv
+        for lo in range(0, F, chunk):
+            f = freqs[lo : lo + chunk]
+            ph = ((2 * np.pi * f)[:, None] * toa[None, :]).astype(LD)
+            S, C = np.sin(ph), np.cos(ph)
+            US, UC = G @ S.T, G @ C.T  # (m, F)
+            vs, vc = aLt @ np.abs(_bwd_ld(L, US)), aLt @ np.abs(_bwd_ld(L, UC))
+            Sn, Cn = S * ninv, C * ninv
+            inner = dict(Mss=(S * Sn).sum(1) - (US * US).sum(0), Msc=(S * Cn).sum(1) - (US * UC).sum(0),
+                         Mcc=(C * Cn).sum(1) - (UC * UC).sum(0), Ns=S @ rn - US.T @ ur, Nc=C @ rn - UC.T @ ur)
+            x0, x1 = _solve_2x2(inner)
+            c = _first_order(x0, x1, vs.T @ vr, vc.T @ vr, (vs * vs).sum(0), (vs * vc).sum(0), (vc * vc).sum(0))
+            out[p, lo : lo + chunk] = c.astype(np.float64)
+    return out
 
 
 def fp_sweep_truth(freqs, toas, residuals, Nvecs, Ts, sigmas, chunk=128):
@@ -259,6 +316,35 @@ def fe_truth_from_inner(inner, freqs, fplus, fcross):
     fe[:, bad] = np.nan
     cond[:, bad] = np.nan
     return fe, cond.astype(np.float64)
+
+
+_PI = LD("3.14159265358979323846264338327950288")
+_FYR = LD(1) / LD(31557600)
+
+
+def _powerlaw_phi_ld(Ffreqs, log10_A, gamma):
+    """``(D, m)`` longdouble power law of ``Ffreqs`` for ``(D,)`` parameters (see :func:`powerlaw_phiinv_truth`)."""
+    f = np.asarray(Ffreqs, dtype=np.float64).astype(LD)
+    df = np.repeat(np.diff(np.concatenate((np.zeros(1, dtype=LD), f[::2]))), 2)[: f.shape[0]]
+    A = np.atleast_1d(np.asarray(log10_A, dtype=np.float64)).astype(LD)[:, None]
+    g = np.atleast_1d(np.asarray(gamma, dtype=np.float64)).astype(LD)[:, None]
+    amp = np.power(LD(10), A)
+    return np.power(f, -g) * (amp * amp) / 12 / (_PI * _PI) * np.power(_FYR, g - 3) * df
+
+
+def powerlaw_phiinv_truth(Ffreqs, log10_A, gamma, curn_Ffreqs=None, curn_log10_A=None, curn_gamma=None):
+    """Truth for the per-draw block of ``RN_container.get_phiinv``: ``(D, m)`` longdouble ``1/phi``.
+
+    ``phi = f^-gamma (10^log10_A)^2 / 12 / pi^2 fyr^(gamma - 3) df`` with ``df = repeat(diff([0, Ffreqs[::2]]), 2)``
+    (reference ``fastfp/nmfp.py:226-234``), plus the common process's power law of ``curn_Ffreqs`` on the leading
+    entries (``:247, 275``), then ``1/phi`` (``:315``). ``log10_A`` / ``gamma`` are ``(D,)`` (or scalars), the CURN
+    ones ``(D,)``. The float64 inputs are exact; everything after them, ``gamma - 3``, ``pi`` and ``fyr = 1 / 31557600``
+    included, is longdouble."""
+    phi = _powerlaw_phi_ld(Ffreqs, log10_A, gamma)
+    if curn_Ffreqs is not None and len(curn_Ffreqs):
+        c = _powerlaw_phi_ld(curn_Ffreqs, curn_log10_A, curn_gamma)
+        phi[:, : c.shape[1]] += c
+    return LD(1) / phi
 
 
 def fe_truth(freqs, fplus, fcross, toas, residuals, Nvecs, Ts, sigmas, blocks=None):
