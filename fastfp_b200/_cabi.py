@@ -163,10 +163,16 @@ def _int64_array(vals: Sequence[int]):
     return (C.c_int64 * len(vals))(*[int(v) for v in vals])
 
 
+def _is_cuda_tensor(x) -> bool:
+    return type(x).__module__.startswith("torch") and getattr(x, "is_cuda", False)
+
+
 def _vp(x) -> C.c_void_p:
-    """host ndarray / integer device address -> void*"""
+    """host ndarray / CUDA tensor / integer device address -> void*"""
     if isinstance(x, np.ndarray):
         return C.c_void_p(x.ctypes.data)
+    if _is_cuda_tensor(x):
+        return C.c_void_p(x.data_ptr())
     return C.c_void_p(int(x))
 
 
@@ -316,12 +322,16 @@ class Pack:
     # -- sweeps -------------------------------------------------------------------------
     @staticmethod
     def _stage(freqs, out, rows=None):
-        """``freqs``: host ndarray or ``(device_address, F)``; ``out``: None (a host array of shape ``(F,)`` or
-        ``(rows, F)`` is allocated and returned), a host ndarray, or an integer device address. Returns the frequency
-        and output arguments (kept alive by the caller), ``F``, the array to return and the location flags."""
+        """``freqs``: host ndarray, contiguous CUDA tensor or ``(device_address, F)``; ``out``: None (a host array of
+        shape ``(F,)`` or ``(rows, F)`` is allocated and returned), a host ndarray, a contiguous CUDA tensor, or an
+        integer device address. Returns the frequency and output arguments (kept alive by the caller), ``F``, the array
+        to return and the location flags."""
         flags = 0
         if isinstance(freqs, tuple):
             freqs, F = freqs
+            flags |= FREQS_ON_DEVICE
+        elif _is_cuda_tensor(freqs):
+            F = freqs.numel()
             flags |= FREQS_ON_DEVICE
         else:
             freqs = as_f64(freqs).reshape(-1)
@@ -333,9 +343,15 @@ class Pack:
             flags |= OUT_ON_DEVICE
         return freqs, out, F, ret, flags
 
+    def _sky(self, fplus, fcross):
+        fplus, fcross = as_f64(fplus), as_f64(fcross)
+        if fplus.ndim != 2 or fplus.shape != fcross.shape or fplus.shape[1] != self.P:
+            raise ValueError("fplus and fcross must both have shape (n_sky, n_pulsars)")
+        return fplus, fcross, fplus.shape[0]
+
     def fp_sweep(self, freqs, out=None, stream: int = 0, terms: bool = False):
-        """``freqs``: host ndarray or ``(device_address, F)``; ``out``: None (a host array is
-        returned), a host ndarray, or an integer device address."""
+        """``freqs``: host ndarray, CUDA tensor or ``(device_address, F)``; ``out``: None (a host array is
+        returned), a host ndarray, a CUDA tensor, or an integer device address."""
         freqs, out, F, ret, flags = self._stage(freqs, out, self.P if terms else None)
         fn = load().fastfp_fp_terms if terms else load().fastfp_fp_sweep
         check(fn(self._h, _vp(freqs), F, _vp(out), flags, C.c_void_p(stream)))
@@ -344,10 +360,7 @@ class Pack:
     def fe_sweep(self, freqs, fplus, fcross, out=None, stream: int = 0):
         """Fe-statistic for ``S`` sky positions: ``fplus``, ``fcross`` host arrays ``(S, P)``; returns / fills
         ``(S, F)``. ``freqs`` / ``out`` as in :meth:`fp_sweep`."""
-        fplus, fcross = as_f64(fplus), as_f64(fcross)
-        if fplus.ndim != 2 or fplus.shape != fcross.shape or fplus.shape[1] != self.P:
-            raise ValueError("fplus and fcross must both have shape (n_sky, n_pulsars)")
-        S = fplus.shape[0]
+        fplus, fcross, S = self._sky(fplus, fcross)
         freqs, out, F, ret, flags = self._stage(freqs, out, S)
         check(load().fastfp_fe_sweep(self._h, _vp(freqs), F, _vp(fplus), _vp(fcross), S, _vp(out), flags,
                                      C.c_void_p(stream)))
@@ -356,7 +369,8 @@ class Pack:
     def fe_skymax(self, freqs, fplus, fcross, out=None, index_out=None, stream: int = 0):
         """Loudest of ``S`` sky positions per frequency: ``fplus``, ``fcross`` host arrays ``(S, P)``. Returns / fills
         ``(fe_max, sky_index)``, ``(F,)`` float64 and int64. ``freqs`` / ``out`` as in :meth:`fp_sweep`; ``index_out``
-        is a host int64 array when ``out`` is on the host, a device address when ``out`` is one."""
+        is a host int64 array when ``out`` is on the host, a CUDA tensor or device address when ``out`` is on the
+        device."""
         return self._skymax(load().fastfp_fe_skymax, None, freqs, fplus, fcross, out, index_out, stream)
 
     def fe_skymax_residuals(self, freqs, fplus, fcross, out=None, index_out=None, stream: int = 0):
@@ -365,10 +379,7 @@ class Pack:
         return self._skymax(load().fastfp_fe_skymax_residuals, self.R, freqs, fplus, fcross, out, index_out, stream)
 
     def _skymax(self, fn, rows, freqs, fplus, fcross, out, index_out, stream):
-        fplus, fcross = as_f64(fplus), as_f64(fcross)
-        if fplus.ndim != 2 or fplus.shape != fcross.shape or fplus.shape[1] != self.P:
-            raise ValueError("fplus and fcross must both have shape (n_sky, n_pulsars)")
-        S = fplus.shape[0]
+        fplus, fcross, S = self._sky(fplus, fcross)
         freqs, out, F, ret, flags = self._stage(freqs, out, rows)
         shape = (F,) if rows is None else (rows, F)
         iret = None

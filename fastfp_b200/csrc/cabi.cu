@@ -118,15 +118,7 @@ static int pack_layout(fastfp_pack* pk, int P, const int64_t* n, const int64_t* 
   FFP_CUDA(cudaMalloc(&pk->d_slab, slab_bytes));
   FFP_CUDA(cudaMalloc(&pk->d_counter, sizeof(unsigned int)));
   pk->bytes = pk_off * 8 + L_off * 8 + (int64_t)sizeof(PulsarMeta) * P + (int64_t)slab_bytes;
-  for (auto& kv : groups) {
-    Group g;
-    g.cfg = kv.first;
-    g.count = (int)kv.second.size();
-    FFP_CUDA(cudaMalloc(&g.d_pidx, sizeof(int) * g.count));
-    FFP_CUDA(cudaMemcpy(g.d_pidx, kv.second.data(), sizeof(int) * g.count, cudaMemcpyHostToDevice));
-    pk->groups.push_back(g);
-  }
-  return 0;
+  return upload_groups(groups, &pk->groups);
 }
 
 // which: 0 = length n_p, 1 = n_p*m_p (T), 2 = m_p*m_p
@@ -170,12 +162,11 @@ static void pack_free(fastfp_pack* pk) {
   for (auto& gr : pk->groups) { cudaFree(gr.d_pidx); cudaFree(gr.d_pidx_rest); }
   cudaFree(pk->d_meta); cudaFree(pk->d_packets); cudaFree(pk->d_L); cudaFree(pk->d_info);
   cudaFree(pk->d_S0); cudaFree(pk->d_zr); cudaFree(pk->d_slab); cudaFree(pk->d_counter); cudaFree(pk->d_done_mask);
-  cudaFree(pk->d_terms); cudaFree(pk->d_freqs); cudaFree(pk->d_out); cudaFree(pk->d_scratch); cudaFree(pk->d_lf);
   cudaFree(pk->d_pl); cudaFreeHost(pk->h_pl);
-  cudaFree(pk->d_i8); cudaFree(pk->d_i8_scale); cudaFree(pk->d_pidx_all); cudaFree(pk->d_inner);
+  cudaFree(pk->d_i8); cudaFree(pk->d_i8_scale); cudaFree(pk->d_pidx_all);
   if (pk->pl_event) cudaEventDestroy(pk->pl_event);
   res_release(pk);
-  delete pk;
+  delete pk;  // and with it the pack's scratch, while its device is current
 }
 
 struct BlockNHost {  // host side arrays of a block-diagonal N (fastfp_pack_create_blockn)
@@ -250,10 +241,10 @@ static int build_pack(int device, int P, const int64_t* n, const int64_t* m, con
   return FASTFP_OK;
 }
 
-// The start of every call that runs work on a pack. While it lives the pack's device is current; select() reports
-// FASTFP_ERR_CUDA if it could not be made so. stage() also resolves the device addresses of the F frequencies (the
-// caller's pointer, or the host array copied into pk->d_freqs) and of the nout result doubles (the caller's pointer,
-// or the pack-owned buffer *buf that the caller copies back to host memory).
+// The start and end of every call that runs work on a pack. While it lives the pack's device is current; select()
+// reports FASTFP_ERR_CUDA if it could not be made so. stage() also resolves the device addresses of the F frequencies
+// (the caller's pointer, or the host array copied into pk->freqs) and of the nout result doubles (the caller's pointer,
+// or the pack-owned buffer *buf that finish() copies back to host memory).
 struct PackCall {
   const fastfp_pack* pk;
   cudaStream_t st;
@@ -265,20 +256,60 @@ struct PackCall {
     return FASTFP_ERR_CUDA;
   }
   int stage(const double* freqs, int64_t F, double* out, int64_t nout, int flags, const double** d_freqs,
-            double** d_out, double** buf, int64_t* cap) const {
+            double** d_out, Scratch<double>* buf) const {
     if (int rc = select()) return rc;
     *d_freqs = freqs;
     if (!(flags & FASTFP_FREQS_ON_DEVICE)) {
-      if (int rc = ensure(&pk->d_freqs, &pk->freqs_cap, F)) return rc;
-      FFP_CUDA(cudaMemcpyAsync(pk->d_freqs, freqs, (size_t)F * 8, cudaMemcpyHostToDevice, st));
-      *d_freqs = pk->d_freqs;
+      if (int rc = pk->freqs.grow(F)) return rc;
+      FFP_CUDA(cudaMemcpyAsync(pk->freqs.get(), freqs, (size_t)F * 8, cudaMemcpyHostToDevice, st));
+      *d_freqs = pk->freqs.get();
     }
     *d_out = out;
     if (!(flags & FASTFP_OUT_ON_DEVICE)) {
-      if (int rc = ensure(buf, cap, nout)) return rc;
-      *d_out = *buf;
+      if (int rc = buf->grow(nout)) return rc;
+      *d_out = buf->get();
     }
     return FASTFP_OK;
+  }
+  // The antenna patterns fplus / fcross, n doubles each, into the scratch at d_fp / d_fx. They are read from memory the
+  // caller owns and may change or free once the call returns, so every Fe call synchronises before it returns, even
+  // when its outputs stay on the device.
+  int upload_sky(const double* fplus, const double* fcross, int64_t n, double* d_fp, double* d_fx) const {
+    FFP_CUDA(cudaMemcpyAsync(d_fp, fplus, (size_t)n * 8, cudaMemcpyHostToDevice, st));
+    FFP_CUDA(cudaMemcpyAsync(d_fx, fcross, (size_t)n * 8, cudaMemcpyHostToDevice, st));
+    return FASTFP_OK;
+  }
+  // Copies the n result doubles d_out (and the n indices d_idx, if the call has them) to the caller's host memory
+  // unless FASTFP_OUT_ON_DEVICE says they stay where they are, then waits for the stream: always after such a copy,
+  // and with outputs on the device only if `always`.
+  int finish(int flags, int64_t n, double* out, const double* d_out, bool always, int64_t* idx = nullptr,
+             const int64_t* d_idx = nullptr) const {
+    const bool to_host = !(flags & FASTFP_OUT_ON_DEVICE);
+    if (to_host) {
+      FFP_CUDA(cudaMemcpyAsync(out, d_out, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
+      if (idx) FFP_CUDA(cudaMemcpyAsync(idx, d_idx, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
+    }
+    if (to_host || always) FFP_CUDA(cudaStreamSynchronize(st));
+    return FASTFP_OK;
+  }
+};
+
+// Frequencies are processed in batches so the per-batch scratch (terms or inner products) stays bounded.
+static const int64_t kTermBudgetDoubles = 1LL << 27;  // 1 GiB
+
+// frequencies per batch of a sweep whose scratch holds doubles_per_freq doubles per frequency: at least 1024
+static int64_t freq_batch(int64_t F, int64_t doubles_per_freq) {
+  return std::max<int64_t>(1024, std::min<int64_t>(F, kTermBudgetDoubles / doubles_per_freq));
+}
+
+// Offsets of the regions of one scratch buffer, taken in the order they are laid out, in 8-byte slots (doubles or
+// int64); total is what the buffer must hold.
+struct ScratchLayout {
+  int64_t total = 0;
+  int64_t take(int64_t n) {
+    const int64_t at = total;
+    total += n;
+    return at;
   }
 };
 
@@ -382,9 +413,6 @@ int fastfp_pack_factor_info(const fastfp_pack_t* pack, int32_t* info) {
   return bad;
 }
 
-// Frequencies are processed in batches so the (P, F_batch) term buffer stays bounded.
-static const int64_t kTermBudgetDoubles = 1LL << 27;  // 1 GiB
-
 static int fp_run(const fastfp_pack* pk, const double* freqs, int64_t F, double* out, int flags,
                   void* stream, bool want_terms) {
   if (!pk || (F > 0 && (!freqs || !out)) || F < 0) {
@@ -398,25 +426,19 @@ static int fp_run(const fastfp_pack* pk, const double* freqs, int64_t F, double*
   PackCall c(pk, stream);
   const double* d_freqs;
   double* d_out;
-  if (int rc = c.stage(freqs, F, out, nout, flags, &d_freqs, &d_out, want_terms ? &pk->d_terms : &pk->d_out,
-                       want_terms ? &pk->terms_cap : &pk->out_cap))
-    return rc;
+  if (int rc = c.stage(freqs, F, out, nout, flags, &d_freqs, &d_out, want_terms ? &pk->terms : &pk->out)) return rc;
   if (want_terms) {
     if (int rc = launch_sweep(pk, d_freqs, F, d_out, c.st)) return rc;
   } else {
-    const int64_t FB = std::max<int64_t>(1024, std::min<int64_t>(F, kTermBudgetDoubles / P));
-    if (int rc = ensure(&pk->d_terms, &pk->terms_cap, (int64_t)P * std::min(FB, F))) return rc;
+    const int64_t FB = freq_batch(F, P);
+    if (int rc = pk->terms.grow((int64_t)P * std::min(FB, F))) return rc;
     for (int64_t lo = 0; lo < F; lo += FB) {
       const int64_t fb = std::min(FB, F - lo);
-      if (int rc = launch_sweep(pk, d_freqs + lo, fb, pk->d_terms, c.st)) return rc;
-      if (int rc = launch_reduce_terms(pk->d_terms, P, fb, d_out + lo, c.st)) return rc;
+      if (int rc = launch_sweep(pk, d_freqs + lo, fb, pk->terms.get(), c.st)) return rc;
+      if (int rc = launch_reduce_terms(pk->terms.get(), P, fb, d_out + lo, c.st)) return rc;
     }
   }
-  if (!(flags & FASTFP_OUT_ON_DEVICE)) {
-    FFP_CUDA(cudaMemcpyAsync(out, d_out, (size_t)nout * 8, cudaMemcpyDeviceToHost, c.st));
-    FFP_CUDA(cudaStreamSynchronize(c.st));
-  }
-  return FASTFP_OK;
+  return c.finish(flags, nout, out, d_out, false);
 }
 
 int fastfp_fp_sweep(const fastfp_pack_t* pack, const double* freqs, int64_t F, double* out,
@@ -485,19 +507,15 @@ int fastfp_fp_sweep_residuals(const fastfp_pack_t* pk, const double* freqs, int6
   PackCall c(pk, stream);
   const double* d_freqs;
   double* d_out;
-  if (int rc = c.stage(freqs, F, out, R * F, flags, &d_freqs, &d_out, &pk->d_out, &pk->out_cap)) return rc;
-  const int64_t FB = std::max<int64_t>(1024, std::min<int64_t>(F, kTermBudgetDoubles / (R * P)));
-  if (int rc = ensure(&pk->d_res_terms, &pk->res_terms_cap, R * P * std::min(FB, F))) return rc;
+  if (int rc = c.stage(freqs, F, out, R * F, flags, &d_freqs, &d_out, &pk->out)) return rc;
+  const int64_t FB = freq_batch(F, R * P);
+  if (int rc = pk->res_terms.grow(R * P * std::min(FB, F))) return rc;
   for (int64_t lo = 0; lo < F; lo += FB) {
     const int64_t fb = std::min(FB, F - lo);
-    if (int rc = launch_fp_sweep_res(pk, d_freqs + lo, fb, pk->d_res_terms, c.st)) return rc;
-    if (int rc = launch_reduce_terms_rows(pk->d_res_terms, (int)R, P, fb, d_out + lo, F, c.st)) return rc;
+    if (int rc = launch_fp_sweep_res(pk, d_freqs + lo, fb, pk->res_terms.get(), c.st)) return rc;
+    if (int rc = launch_reduce_terms_rows(pk->res_terms.get(), (int)R, P, fb, d_out + lo, F, c.st)) return rc;
   }
-  if (!(flags & FASTFP_OUT_ON_DEVICE)) {
-    FFP_CUDA(cudaMemcpyAsync(out, d_out, (size_t)(R * F) * 8, cudaMemcpyDeviceToHost, c.st));
-    FFP_CUDA(cudaStreamSynchronize(c.st));
-  }
-  return FASTFP_OK;
+  return c.finish(flags, R * F, out, d_out, false);
 }
 
 // Fe-statistic sky scan: one sweep for the inner products of every (pulsar, frequency), then the combine kernel
@@ -513,26 +531,21 @@ int fastfp_fe_sweep(const fastfp_pack_t* pk, const double* freqs, int64_t F, con
   PackCall c(pk, stream);
   const double* d_freqs;
   double* d_out;
-  if (int rc = c.stage(freqs, F, out, S * F, flags, &d_freqs, &d_out, &pk->d_out, &pk->out_cap)) return rc;
-  const int64_t FB = std::max<int64_t>(1024, std::min<int64_t>(F, kTermBudgetDoubles / (5 * (int64_t)P)));
+  if (int rc = c.stage(freqs, F, out, S * F, flags, &d_freqs, &d_out, &pk->out)) return rc;
+  const int64_t FB = freq_batch(F, 5 * (int64_t)P);
   // scratch: the inner products of one frequency batch, then the antenna patterns of the S sky positions
-  if (int rc = ensure(&pk->d_inner, &pk->inner_cap, 5 * (int64_t)P * std::min(FB, F) + 2 * S * P)) return rc;
-  double* d_fp = pk->d_inner + 5 * (int64_t)P * std::min(FB, F);
-  double* d_fx = d_fp + S * P;
-  FFP_CUDA(cudaMemcpyAsync(d_fp, fplus, (size_t)S * P * 8, cudaMemcpyHostToDevice, c.st));
-  FFP_CUDA(cudaMemcpyAsync(d_fx, fcross, (size_t)S * P * 8, cudaMemcpyHostToDevice, c.st));
+  ScratchLayout lay;
+  const int64_t o_inner = lay.take(5 * (int64_t)P * std::min(FB, F)), o_fp = lay.take(S * P), o_fx = lay.take(S * P);
+  if (int rc = pk->inner.grow(lay.total)) return rc;
+  double* base = pk->inner.get();
+  double *d_inner = base + o_inner, *d_fp = base + o_fp, *d_fx = base + o_fx;
+  if (int rc = c.upload_sky(fplus, fcross, S * P, d_fp, d_fx)) return rc;
   for (int64_t lo = 0; lo < F; lo += FB) {
     const int64_t fb = std::min(FB, F - lo);
-    if (int rc = launch_sweep(pk, d_freqs + lo, fb, nullptr, c.st, nullptr, pk->d_inner)) return rc;
-    if (int rc = launch_fe_combine(pk->d_inner, P, fb, d_fp, d_fx, S, d_out + lo, F, c.st)) return rc;
+    if (int rc = launch_sweep(pk, d_freqs + lo, fb, nullptr, c.st, nullptr, d_inner)) return rc;
+    if (int rc = launch_fe_combine(d_inner, P, fb, d_fp, d_fx, S, d_out + lo, F, c.st)) return rc;
   }
-  if (!(flags & FASTFP_OUT_ON_DEVICE)) {
-    FFP_CUDA(cudaMemcpyAsync(out, d_out, (size_t)S * F * 8, cudaMemcpyDeviceToHost, c.st));
-    FFP_CUDA(cudaStreamSynchronize(c.st));
-  } else {
-    FFP_CUDA(cudaStreamSynchronize(c.st));  // fplus / fcross were read from caller-owned host memory
-  }
-  return FASTFP_OK;
+  return c.finish(flags, S * F, out, d_out, true);
 }
 
 // Sky-maximised Fe: the same sweep per frequency batch, then a combine that reduces over the sky as it goes
@@ -549,8 +562,8 @@ int fastfp_fe_skymax(const fastfp_pack_t* pk, const double* freqs, int64_t F, co
   PackCall c(pk, stream);
   const double* d_freqs;
   double* d_max;
-  if (int rc = c.stage(freqs, F, fe_max, F, flags, &d_freqs, &d_max, &pk->d_out, &pk->out_cap)) return rc;
-  const int64_t FB = std::max<int64_t>(1024, std::min<int64_t>(F, kTermBudgetDoubles / (5 * (int64_t)P)));
+  if (int rc = c.stage(freqs, F, fe_max, F, flags, &d_freqs, &d_max, &pk->out)) return rc;
+  const int64_t FB = freq_batch(F, 5 * (int64_t)P);
   const int64_t fb0 = std::min(FB, F);
   const FeSkyPlan plan = fe_skymax_plan(fb0, S, pk->num_sms);
   // scratch, all in the pack's Fe buffer: the inner products of one frequency batch, the antenna patterns and the
@@ -559,30 +572,27 @@ int fastfp_fe_skymax(const fastfp_pack_t* pk, const double* freqs, int64_t F, co
   // until the pack is destroyed: 5 P F_batch + 7 S P doubles, plus F for host outputs and a small split scratch; about
   // 750 MB after a call with S = 196 608 and P = 68. Allocating it per call instead costs a cudaMalloc / cudaFree pair per call, measured at up
   // to several times the whole call at C2 sizes.
-  const int64_t n_inner = 5 * (int64_t)P * fb0, n_part = plan.nchunk > 1 ? plan.nchunk * fb0 : 0;
-  const int64_t n_idx = (flags & FASTFP_OUT_ON_DEVICE) ? 0 : F;
-  if (int rc = ensure(&pk->d_inner, &pk->inner_cap, n_inner + 7 * S * P + 2 * n_part + n_idx)) return rc;
-  double* d_fp = pk->d_inner + n_inner;
-  double* d_fx = d_fp + S * P;
-  double* d_w = d_fx + S * P;
-  double* part_v = d_w + 5 * S * P;
-  int64_t* part_i = reinterpret_cast<int64_t*>(part_v + n_part);
-  int64_t* d_idx = n_idx ? part_i + n_part : sky_index;
-  FFP_CUDA(cudaMemcpyAsync(d_fp, fplus, (size_t)S * P * 8, cudaMemcpyHostToDevice, c.st));
-  FFP_CUDA(cudaMemcpyAsync(d_fx, fcross, (size_t)S * P * 8, cudaMemcpyHostToDevice, c.st));
+  const int64_t n_part = plan.nchunk > 1 ? plan.nchunk * fb0 : 0;
+  const bool idx_to_host = !(flags & FASTFP_OUT_ON_DEVICE);
+  ScratchLayout lay;
+  const int64_t o_inner = lay.take(5 * (int64_t)P * fb0), o_fp = lay.take(S * P), o_fx = lay.take(S * P),
+                o_w = lay.take(5 * S * P), o_part_v = lay.take(n_part), o_part_i = lay.take(n_part),
+                o_idx = lay.take(idx_to_host ? F : 0);
+  if (int rc = pk->inner.grow(lay.total)) return rc;
+  double* base = pk->inner.get();
+  double *d_inner = base + o_inner, *d_fp = base + o_fp, *d_fx = base + o_fx, *d_w = base + o_w;
+  double* part_v = base + o_part_v;
+  int64_t* part_i = reinterpret_cast<int64_t*>(base + o_part_i);
+  int64_t* d_idx = idx_to_host ? reinterpret_cast<int64_t*>(base + o_idx) : sky_index;
+  if (int rc = c.upload_sky(fplus, fcross, S * P, d_fp, d_fx)) return rc;
   if (int rc = launch_fe_sky_weights(d_fp, d_fx, S * P, d_w, c.st)) return rc;
   for (int64_t lo = 0; lo < F; lo += FB) {
     const int64_t fb = std::min(FB, F - lo);
-    if (int rc = launch_sweep(pk, d_freqs + lo, fb, nullptr, c.st, nullptr, pk->d_inner)) return rc;
-    if (int rc = launch_fe_skymax(pk->d_inner, P, fb, d_w, S, plan, part_v, part_i, d_max + lo, d_idx + lo, c.st))
+    if (int rc = launch_sweep(pk, d_freqs + lo, fb, nullptr, c.st, nullptr, d_inner)) return rc;
+    if (int rc = launch_fe_skymax(d_inner, P, fb, d_w, S, plan, part_v, part_i, d_max + lo, d_idx + lo, c.st))
       return rc;
   }
-  if (!(flags & FASTFP_OUT_ON_DEVICE)) {
-    FFP_CUDA(cudaMemcpyAsync(fe_max, d_max, (size_t)F * 8, cudaMemcpyDeviceToHost, c.st));
-    FFP_CUDA(cudaMemcpyAsync(sky_index, d_idx, (size_t)F * 8, cudaMemcpyDeviceToHost, c.st));
-  }
-  FFP_CUDA(cudaStreamSynchronize(c.st));  // fplus / fcross were read from caller-owned host memory
-  return FASTFP_OK;
+  return c.finish(flags, F, fe_max, d_max, true, sky_index, d_idx);
 }
 
 // Sky-maximised Fe of each residual realisation (DESIGN.md section 5e): per frequency batch, the residual sweep writes
@@ -609,37 +619,33 @@ int fastfp_fe_skymax_residuals(const fastfp_pack_t* pk, const double* freqs, int
   PackCall c(pk, stream);
   const double* d_freqs;
   double* d_max;
-  if (int rc = c.stage(freqs, F, fe_max, R * F, flags, &d_freqs, &d_max, &pk->d_out, &pk->out_cap)) return rc;
-  const int64_t FB = std::max<int64_t>(1024, std::min<int64_t>(F, kTermBudgetDoubles / ((2 * R + 3) * P)));
+  if (int rc = c.stage(freqs, F, fe_max, R * F, flags, &d_freqs, &d_max, &pk->out)) return rc;
+  const int64_t FB = freq_batch(F, (2 * R + 3) * P);
   const int64_t fb0 = std::min(FB, F);
   // the sky is split across CTAs only in a single-batch call: the per-chunk bests are merged into (R, F) columns
   const FeSkyPlan plan = fe_skymax_res_plan(fb0, R, S, pk->num_sms, F <= FB);
   // scratch: (s|r_k), (c|r_k) of one frequency batch in the residual terms buffer; in the Fe buffer (s|s), (s|c), (c|c)
   // of the batch, the antenna patterns, the per-chunk bests of a split sky and the indices on their way to host memory
-  const int64_t n_mi = 3 * (int64_t)P * fb0, n_part = plan.nchunk > 1 ? plan.nchunk * R * fb0 : 0;
-  const int64_t n_idx = (flags & FASTFP_OUT_ON_DEVICE) ? 0 : R * F;
-  if (int rc = ensure(&pk->d_res_terms, &pk->res_terms_cap, 2 * R * P * fb0)) return rc;
-  if (int rc = ensure(&pk->d_inner, &pk->inner_cap, n_mi + 2 * S * P + 2 * n_part + n_idx)) return rc;
-  double* d_fp = pk->d_inner + n_mi;
-  double* d_fx = d_fp + S * P;
-  double* part_v = d_fx + S * P;
-  int64_t* part_i = reinterpret_cast<int64_t*>(part_v + n_part);
-  int64_t* d_idx = n_idx ? part_i + n_part : sky_index;
-  FFP_CUDA(cudaMemcpyAsync(d_fp, fplus, (size_t)S * P * 8, cudaMemcpyHostToDevice, c.st));
-  FFP_CUDA(cudaMemcpyAsync(d_fx, fcross, (size_t)S * P * 8, cudaMemcpyHostToDevice, c.st));
+  const int64_t n_part = plan.nchunk > 1 ? plan.nchunk * R * fb0 : 0;
+  const bool idx_to_host = !(flags & FASTFP_OUT_ON_DEVICE);
+  if (int rc = pk->res_terms.grow(2 * R * P * fb0)) return rc;
+  ScratchLayout lay;
+  const int64_t o_mi = lay.take(3 * (int64_t)P * fb0), o_fp = lay.take(S * P), o_fx = lay.take(S * P),
+                o_part_v = lay.take(n_part), o_part_i = lay.take(n_part), o_idx = lay.take(idx_to_host ? R * F : 0);
+  if (int rc = pk->inner.grow(lay.total)) return rc;
+  double* base = pk->inner.get();
+  double *d_mi = base + o_mi, *d_fp = base + o_fp, *d_fx = base + o_fx, *part_v = base + o_part_v;
+  int64_t* part_i = reinterpret_cast<int64_t*>(base + o_part_i);
+  int64_t* d_idx = idx_to_host ? reinterpret_cast<int64_t*>(base + o_idx) : sky_index;
+  if (int rc = c.upload_sky(fplus, fcross, S * P, d_fp, d_fx)) return rc;
   for (int64_t lo = 0; lo < F; lo += FB) {
     const int64_t fb = std::min(FB, F - lo);
-    if (int rc = launch_fp_sweep_res(pk, d_freqs + lo, fb, pk->d_res_terms, c.st, pk->d_inner)) return rc;
-    if (int rc = launch_fe_skymax_res(pk->d_res_terms, pk->d_inner, P, R, fb, d_fp, d_fx, S, plan, part_v, part_i,
+    if (int rc = launch_fp_sweep_res(pk, d_freqs + lo, fb, pk->res_terms.get(), c.st, d_mi)) return rc;
+    if (int rc = launch_fe_skymax_res(pk->res_terms.get(), d_mi, P, R, fb, d_fp, d_fx, S, plan, part_v, part_i,
                                       d_max + lo, d_idx + lo, F, c.st))
       return rc;
   }
-  if (!(flags & FASTFP_OUT_ON_DEVICE)) {
-    FFP_CUDA(cudaMemcpyAsync(fe_max, d_max, (size_t)(R * F) * 8, cudaMemcpyDeviceToHost, c.st));
-    FFP_CUDA(cudaMemcpyAsync(sky_index, d_idx, (size_t)(R * F) * 8, cudaMemcpyDeviceToHost, c.st));
-  }
-  FFP_CUDA(cudaStreamSynchronize(c.st));  // fplus / fcross were read from caller-owned host memory
-  return FASTFP_OK;
+  return c.finish(flags, R * F, fe_max, d_max, true, sky_index, d_idx);
 }
 
 int fastfp_nmfp_sweep(const fastfp_pack_t* pk, const double* freqs, int64_t F,
@@ -653,7 +659,7 @@ int fastfp_nmfp_sweep(const fastfp_pack_t* pk, const double* freqs, int64_t F,
   PackCall c(pk, stream);
   const double* d_freqs;
   double* d_out;
-  if (int rc = c.stage(freqs, F, out, D * F, flags, &d_freqs, &d_out, &pk->d_out, &pk->out_cap)) return rc;
+  if (int rc = c.stage(freqs, F, out, D * F, flags, &d_freqs, &d_out, &pk->out)) return rc;
   const double* d_phi = phiinv_var;
   DeviceBuf<double> d_phi_tmp;
   if (!(flags & FASTFP_PARAMS_ON_DEVICE)) {
@@ -663,11 +669,7 @@ int fastfp_nmfp_sweep(const fastfp_pack_t* pk, const double* freqs, int64_t F,
     d_phi = d_phi_tmp.get();
   }
   int rc = nmfp_sweep_impl(pk, d_freqs, F, d_phi, D, d_out, c.st);
-  if (!rc && !(flags & FASTFP_OUT_ON_DEVICE)) {
-    cudaError_t e = cudaMemcpyAsync(out, d_out, (size_t)D * F * 8, cudaMemcpyDeviceToHost, c.st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c.st);
-    if (e != cudaSuccess) rc = cuda_fail(e, "copy nmfp result to host");
-  }
+  if (!rc) rc = c.finish(flags, D * F, out, d_out, false);
   if (d_phi_tmp) cudaStreamSynchronize(c.st);  // the sweep reads the staged parameters until it ends
   return rc;
 }

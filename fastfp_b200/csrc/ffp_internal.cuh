@@ -5,6 +5,7 @@
 #include <stdint.h>
 
 #include <atomic>
+#include <map>
 #include <memory>
 #include <string>
 #include <vector>
@@ -118,6 +119,49 @@ struct Group {  // pulsars that share one kernel instantiation
   int* d_pidx_rest = nullptr;
 };
 
+extern std::atomic<int64_t> g_launches;
+void set_error(const std::string& msg);
+int cuda_fail(cudaError_t e, const char* what);
+
+#define FFP_CUDA(call)                                         \
+  do {                                                         \
+    cudaError_t e__ = (call);                                  \
+    if (e__ != cudaSuccess) return ffp::cuda_fail(e__, #call); \
+  } while (0)
+
+// device memory a host function holds for one call: cudaFree'd when the holder goes out of scope, on every return path
+struct CudaFree {
+  void operator()(void* p) const { cudaFree(p); }
+};
+template <typename T>
+using DeviceBuf = std::unique_ptr<T, CudaFree>;
+template <typename T>
+inline cudaError_t dev_alloc(DeviceBuf<T>* buf, size_t count) {
+  T* p = nullptr;
+  const cudaError_t e = cudaMalloc(&p, count * sizeof(T));
+  buf->reset(e == cudaSuccess ? p : nullptr);
+  return e;
+}
+
+// device memory a pack keeps for its calls: grown on demand (contents are not preserved), kept until released
+template <typename T>
+struct Scratch {
+  DeviceBuf<T> buf;
+  int64_t cap = 0;
+  T* get() const { return buf.get(); }
+  int grow(int64_t need) {
+    if (cap >= need) return 0;
+    release();  // before the new allocation: the old and the new buffer are never held together
+    FFP_CUDA(dev_alloc(&buf, (size_t)need));
+    cap = need;
+    return 0;
+  }
+  void release() {
+    buf.reset();
+    cap = 0;
+  }
+};
+
 }  // namespace ffp
 
 // The opaque handle of include/fastfp_b200.h.
@@ -157,19 +201,13 @@ struct fastfp_pack {
   // nmfp only
   double* d_S0 = nullptr;  // [P][mvmax][mvmax] Schur complement of the fixed block (no phiinv)
   double* d_zr = nullptr;  // [P][mvmax]  z'_r
-  // scratch reused across sweeps (grown on demand)
-  mutable double* d_terms = nullptr;
-  mutable int64_t terms_cap = 0;
-  mutable double* d_freqs = nullptr;
-  mutable int64_t freqs_cap = 0;
-  mutable double* d_out = nullptr;
-  mutable int64_t out_cap = 0;
-  mutable double* d_scratch = nullptr;  // nmfp: stage-A tiles of a frequency batch
-  mutable int64_t scratch_cap = 0;
-  mutable double* d_lf = nullptr;       // nmfp: L^-1 fragments of a draw batch
-  mutable int64_t lf_cap = 0;
-  mutable double* d_inner = nullptr;   // Fe-statistic: inner products of a frequency batch + antenna patterns
-  mutable int64_t inner_cap = 0;
+  // scratch reused across sweeps
+  mutable ffp::Scratch<double> terms;
+  mutable ffp::Scratch<double> freqs;
+  mutable ffp::Scratch<double> out;
+  mutable ffp::Scratch<double> scratch;  // nmfp: stage-A tiles of a frequency batch
+  mutable ffp::Scratch<double> lf;       // nmfp: L^-1 fragments of a draw batch
+  mutable ffp::Scratch<double> inner;    // Fe-statistic: inner products of a frequency batch + antenna patterns
   // staging of the per-draw power-law parameters (fastfp_powerlaw_phiinv): device + pinned host copy,
   // the event marks the last H2D copy out of h_pl; pl_tab is the frequency table already on the device
   mutable double* d_pl = nullptr;
@@ -184,50 +222,13 @@ struct fastfp_pack {
   double* d_res_packets = nullptr;
   ffp::PulsarMeta* d_res_meta = nullptr;
   std::vector<ffp::Group> res_groups;
-  mutable double* d_res_terms = nullptr;  // [R][P][F_batch] terms of one frequency batch
-  mutable int64_t res_terms_cap = 0;
+  mutable ffp::Scratch<double> res_terms;  // [R][P][F_batch] terms of one frequency batch
   // optional per-stage timing of nmfp sweeps (fastfp_nmfp_stage_timing): stage A, factor, stage B
   mutable bool time_stages = false;
   mutable double stage_ms[3] = {0.0, 0.0, 0.0};
 };
 
 namespace ffp {
-
-extern std::atomic<int64_t> g_launches;
-void set_error(const std::string& msg);
-int cuda_fail(cudaError_t e, const char* what);
-
-#define FFP_CUDA(call)                                         \
-  do {                                                         \
-    cudaError_t e__ = (call);                                  \
-    if (e__ != cudaSuccess) return ffp::cuda_fail(e__, #call); \
-  } while (0)
-
-// grow-on-demand device scratch (contents are not preserved)
-template <typename T>
-inline int ensure(T** buf, int64_t* cap, int64_t need) {
-  if (*cap >= need) return 0;
-  if (*buf) cudaFree(*buf);
-  *buf = nullptr;
-  *cap = 0;
-  FFP_CUDA(cudaMalloc(buf, (size_t)need * sizeof(T)));
-  *cap = need;
-  return 0;
-}
-
-// device memory a host function holds for one call: cudaFree'd when the holder goes out of scope, on every return path
-struct CudaFree {
-  void operator()(void* p) const { cudaFree(p); }
-};
-template <typename T>
-using DeviceBuf = std::unique_ptr<T, CudaFree>;
-template <typename T>
-inline cudaError_t dev_alloc(DeviceBuf<T>* buf, size_t count) {
-  T* p = nullptr;
-  const cudaError_t e = cudaMalloc(&p, count * sizeof(T));
-  buf->reset(e == cudaSuccess ? p : nullptr);
-  return e;
-}
 
 // ---- kernel launchers (defined in the .cu files) ---------------------------------------
 // precompute.cu
@@ -244,6 +245,8 @@ int launch_fp_precompute(fastfp_pack* pk, const double* d_toas, const double* d_
 // set. res_release frees them (R = 0).
 int build_res_packets(fastfp_pack* pk, int64_t R, const double* d_res, cudaStream_t st);
 void res_release(fastfp_pack* pk);
+// the pulsars of each kernel configuration as Groups with their indices on the device, appended to *out
+int upload_groups(const std::map<KernelCfg, std::vector<int>>& groups, std::vector<Group>* out);
 // fp_sweep*.cu
 struct NmfpOut {      // stage-A outputs of the nmfp path (null for plain Fp)
   double* Z;          // [P][ceil(F/32)][mvpad/4][8][32]  z'_s, z'_c tiles in MMA B-fragment order

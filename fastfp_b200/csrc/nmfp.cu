@@ -655,8 +655,8 @@ int nmfp_stage_b_impl(const fastfp_pack* pk, const double* d_freqs, int64_t F, c
     }
     DB = std::min<int64_t>(std::max<int64_t>(NB_DT, groups * NB_DT), std::max<int64_t>(NB_DT, (D + NB_DT - 1) / NB_DT * NB_DT));
   }
-  if (int rc = ensure(&pk->d_lf, &pk->lf_cap, DB * P * lfw)) return rc;
-  double* dLf = pk->d_lf;
+  if (int rc = pk->lf.grow(DB * P * lfw)) return rc;
+  double* dLf = pk->lf.get();
   for (int64_t dd = 0; dd < D; dd += DB) {
     const int Db = (int)std::min(DB, D - dd);
     StageBArgs sb{dZ, dA, dLf, d_freqs, pk->d_meta, d_out + dd * out_ld, F, out_ld, P, nt32, Db, lfw, nt_blk};
@@ -685,8 +685,8 @@ int nmfp_sweep_impl(const fastfp_pack* pk, const double* d_freqs, int64_t F, con
   int64_t FB = std::max<int64_t>(32, ((1LL << 27) / std::max<int64_t>(1, per_f32)) * 32);
   FB = std::min<int64_t>(FB, (F + 31) / 32 * 32);
   const int64_t nt32_max = FB / 32;
-  if (int rc = ensure(&pk->d_scratch, &pk->scratch_cap, P * nt32_max * (int64_t)(MV * 64 + 160))) return rc;
-  double* dZ = pk->d_scratch;
+  if (int rc = pk->scratch.grow(P * nt32_max * (int64_t)(MV * 64 + 160))) return rc;
+  double* dZ = pk->scratch.get();
   double* dA = dZ + P * nt32_max * (int64_t)MV * 64;
   StageMarks marks;
   marks.on = pk->time_stages;

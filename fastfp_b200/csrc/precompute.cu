@@ -273,16 +273,26 @@ __global__ void __launch_bounds__(256) w_batch_kernel(double* __restrict__ rpk, 
       g_frag_index(i % CI, ((pm.m + 7) & ~7) + k, rm.mpad >> 3)] = w;
 }
 
+int upload_groups(const std::map<KernelCfg, std::vector<int>>& groups, std::vector<Group>* out) {
+  for (auto& kv : groups) {
+    Group g;
+    g.cfg = kv.first;
+    g.count = (int)kv.second.size();
+    FFP_CUDA(cudaMalloc(&g.d_pidx, sizeof(int) * g.count));
+    out->push_back(g);  // before the copy, so that the owner frees it if the copy fails
+    FFP_CUDA(cudaMemcpy(g.d_pidx, kv.second.data(), sizeof(int) * g.count, cudaMemcpyHostToDevice));
+  }
+  return 0;
+}
+
 void res_release(fastfp_pack* pk) {
   for (auto& g : pk->res_groups) cudaFree(g.d_pidx);
   pk->res_groups.clear();
   cudaFree(pk->d_res_packets);
   cudaFree(pk->d_res_meta);
-  cudaFree(pk->d_res_terms);
   pk->d_res_packets = nullptr;
   pk->d_res_meta = nullptr;
-  pk->d_res_terms = nullptr;
-  pk->res_terms_cap = 0;
+  pk->res_terms.release();
   pk->res_R = 0;
   pk->res_bytes = 0;
 }
@@ -313,14 +323,7 @@ int build_res_packets(fastfp_pack* pk, int64_t R, const double* d_res, cudaStrea
   FFP_CUDA(cudaMalloc(&pk->d_res_meta, sizeof(PulsarMeta) * P));
   FFP_CUDA(cudaMemcpy(pk->d_res_meta, rmeta.data(), sizeof(PulsarMeta) * P, cudaMemcpyHostToDevice));
   FFP_CUDA(cudaMalloc(&pk->d_res_packets, (size_t)off * 8));
-  for (auto& kv : groups) {
-    Group g;
-    g.cfg = kv.first;
-    g.count = (int)kv.second.size();
-    FFP_CUDA(cudaMalloc(&g.d_pidx, sizeof(int) * g.count));
-    pk->res_groups.push_back(g);
-    FFP_CUDA(cudaMemcpy(g.d_pidx, kv.second.data(), sizeof(int) * g.count, cudaMemcpyHostToDevice));
-  }
+  if (int rc = upload_groups(groups, &pk->res_groups)) return rc;
   pk->res_bytes = off * 8 + (int64_t)sizeof(PulsarMeta) * P;
   DeviceBuf<double> U;
   FFP_CUDA(dev_alloc(&U, (size_t)P * R * mmax));

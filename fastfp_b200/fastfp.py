@@ -22,6 +22,7 @@ import os
 import numpy as np
 
 from . import _cabi
+from ._cabi import _is_cuda_tensor
 
 
 def _fingerprint(lists) -> tuple:
@@ -124,6 +125,22 @@ class _PackCache:
             raise ValueError(f"fgw is on {fgw.device}, the pack on cuda:{self.device}")
         return fgw.contiguous().reshape(-1), torch.cuda.current_stream(fgw.device).cuda_stream
 
+    def _front_end(self, fgw):
+        """What a front end hands the pack for ``fgw``: the flat float64 frequencies, ``empty(shape, dtype=float64)``
+        for its outputs, the stream and whether the call is asynchronous. A CUDA tensor stays on its device: outputs
+        from ``torch.empty`` there, torch's current stream, asynchronous. Host values: ``np.empty``, stream 0, and the
+        call returns with the results on the host."""
+        if _is_cuda_tensor(fgw):
+            import torch
+
+            f, stream = self._device_freqs(fgw)
+
+            def empty(shape, dtype=np.float64):
+                return torch.empty(shape, dtype=getattr(torch, np.dtype(dtype).name), device=f.device)
+
+            return f, empty, stream, True
+        return np.asarray(fgw, dtype=np.float64).reshape(-1), np.empty, 0, False
+
     def _ensure(self, lists, force=False, key=None):
         key = _fingerprint(lists) if key is None else key
         if force or self._pack is None or key != self._pack_key:
@@ -182,10 +199,6 @@ def batch_pass_rows(R: int, m) -> int:
     return best[2]
 
 
-def _is_cuda_tensor(x) -> bool:
-    return type(x).__module__.startswith("torch") and getattr(x, "is_cuda", False)
-
-
 class FastFp(_PackCache):
     """Fp-statistic (Ellis, Siemens & Creighton 2012) for a list of pulsars.
 
@@ -222,21 +235,15 @@ class FastFp(_PackCache):
     def calculate_Fp(self, fgw, Nvecs, Ts, sigmas):
         """Fp at ``fgw`` (reference ``fastfp.py:51-92``); see the module docstring for the
         batched forms of ``fgw``."""
-        lists = (Nvecs, Ts, sigmas)
-        if _is_cuda_tensor(fgw):
-            import torch
+        f, empty, stream, on_device = self._front_end(fgw)
+        out = empty(f.shape[0])
 
-            f, stream = self._device_freqs(fgw)
-            out = torch.empty(f.shape[0], dtype=torch.float64, device=f.device)
+        def run(pack):
+            pack.fp_sweep(f, out=out, stream=stream)
+            return out
 
-            def run(pack):
-                pack.fp_sweep((f.data_ptr(), f.shape[0]), out=out.data_ptr(), stream=stream)
-                return out
-
-            return self._run_verified(lists, run, asynchronous=True).reshape(fgw.shape)
-        f = np.asarray(fgw, dtype=np.float64)
-        res = self._run_verified(lists, lambda pack: pack.fp_sweep(f.reshape(-1)), asynchronous=False)
-        return np.float64(res[0]) if f.ndim == 0 else res.reshape(f.shape)
+        res = self._run_verified((Nvecs, Ts, sigmas), run, asynchronous=on_device)
+        return res.reshape(np.shape(fgw))[()]  # a scalar fgw: a numpy scalar from host values, a 0-d tensor from a tensor
 
     compute_Fp = calculate_Fp
 
@@ -258,30 +265,15 @@ class FastFp(_PackCache):
         sweep cost (measured per-row costs of the kernel configurations). The pass size selects the kernel configuration, so values can differ in the last bits
         between different ``R``; within one ``R`` every row is computed alike wherever it sits."""
         R, passes = self._residual_passes(residuals)
-        lists = (Nvecs, Ts, sigmas)
-
-        if _is_cuda_tensor(fgw):
-            import torch
-
-            f, stream = self._device_freqs(fgw)
-            out = torch.empty((R, f.shape[0]), dtype=torch.float64, device=f.device)
-
-            def run(pack):
-                for lo, _ in passes(pack, stream):
-                    pack.fp_sweep_residuals((f.data_ptr(), f.shape[0]), out=out[lo].data_ptr(), stream=stream)
-                return out
-
-            return self._run_verified(lists, run, asynchronous=True).reshape((R,) + tuple(fgw.shape))
-        f = np.asarray(fgw, dtype=np.float64)
-        fl = f.reshape(-1)
+        f, empty, stream, on_device = self._front_end(fgw)
+        out = empty((R, f.shape[0]))
 
         def run(pack):
-            out = np.empty((R, fl.shape[0]))
-            for lo, hi in passes(pack):
-                pack.fp_sweep_residuals(fl, out=out[lo:hi])
+            for lo, hi in passes(pack, stream):
+                pack.fp_sweep_residuals(f, out=out[lo:hi], stream=stream)
             return out
 
-        return self._run_verified(lists, run, asynchronous=False).reshape((R,) + f.shape)
+        return self._run_verified((Nvecs, Ts, sigmas), run, asynchronous=on_device).reshape((R,) + np.shape(fgw))
 
     def _residual_passes(self, residuals):
         """Checks the shapes of ``residuals`` (a list of ``P`` arrays ``(R, n_p)``) and returns ``(R, passes)``:

@@ -12,7 +12,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from .fastfp import FastFp, _is_cuda_tensor
+from .fastfp import FastFp
 
 
 def antenna_pattern(pos, gwtheta, gwphi):
@@ -42,31 +42,18 @@ class FastFe(FastFp):
         """Fe at frequency ``fgw`` (scalar or ``(F,)``, host array or CUDA tensor) and sky position(s)
         ``gwtheta``, ``gwphi`` (scalars or ``(S,)``): returns a scalar, ``(F,)``, ``(S,)`` or ``(S, F)``. A frequency
         ``f <= 0`` gives NaN, as in :meth:`calculate_Fp` (the reference's ``f^(-1/3)``)."""
-        th, ph = np.asarray(gwtheta, dtype=np.float64), np.asarray(gwphi, dtype=np.float64)
-        sky_batched = th.ndim > 0 or ph.ndim > 0
-        th, ph = np.broadcast_arrays(np.atleast_1d(th), np.atleast_1d(ph))
-        fplus, fcross = antenna_pattern(self.pos, th, ph)  # (S, P)
-        lists = (Nvecs, Ts, sigmas)
-        if _is_cuda_tensor(fgw):
-            import torch
+        sky_batched = np.ndim(gwtheta) > 0 or np.ndim(gwphi) > 0
+        fplus, fcross = self._sky_grid(gwtheta, gwphi)
+        f, empty, stream, on_device = self._front_end(fgw)
+        out = empty((fplus.shape[0], f.shape[0]))
 
-            f, stream = self._device_freqs(fgw)
-            out = torch.empty((fplus.shape[0], f.shape[0]), dtype=torch.float64, device=f.device)
+        def run(pack):
+            pack.fe_sweep(f, fplus, fcross, out=out, stream=stream)
+            return out
 
-            def run(pack):
-                pack.fe_sweep((f.data_ptr(), f.shape[0]), fplus, fcross, out=out.data_ptr(), stream=stream)
-                return out
-
-            res = self._run_verified(lists, run, asynchronous=True)
-            res = res if fgw.ndim else res[:, 0]
-            return res if sky_batched else res[0]
-        f = np.asarray(fgw, dtype=np.float64)
-        res = self._run_verified(lists, lambda pack: pack.fe_sweep(f.reshape(-1), fplus, fcross), asynchronous=False)
-        if f.ndim == 0:
-            res = res[:, 0]
-        if not sky_batched:
-            res = res[0]
-        return np.float64(res) if np.ndim(res) == 0 else res
+        res = self._run_verified((Nvecs, Ts, sigmas), run, asynchronous=on_device)
+        res = res if np.ndim(fgw) else res[:, 0]
+        return res if sky_batched else res[0]
 
     compute_Fe = calculate_Fe
 
@@ -78,27 +65,17 @@ class FastFe(FastFp):
         CUDA tensor. Each value equals the corresponding entry of :meth:`calculate_Fe`'s map bit for bit; NaN loses,
         ties go to the lowest index, and a frequency with no finite value gives ``(nan, -1)``."""
         fplus, fcross = self._sky_grid(gwtheta, gwphi)
-        lists = (Nvecs, Ts, sigmas)
-        if _is_cuda_tensor(fgw):
-            import torch
+        f, empty, stream, on_device = self._front_end(fgw)
+        best, idx = empty(f.shape[0]), empty(f.shape[0], np.int64)
 
-            f, stream = self._device_freqs(fgw)
-            best = torch.empty(f.shape[0], dtype=torch.float64, device=f.device)
-            idx = torch.empty(f.shape[0], dtype=torch.int64, device=f.device)
+        def run(pack):
+            pack.fe_skymax(f, fplus, fcross, out=best, index_out=idx, stream=stream)
+            return best, idx
 
-            def run(pack):
-                pack.fe_skymax((f.data_ptr(), f.shape[0]), fplus, fcross, out=best.data_ptr(),
-                               index_out=idx.data_ptr(), stream=stream)
-                return best, idx
-
-            best, idx = self._run_verified(lists, run, asynchronous=True)
-            return best.reshape(fgw.shape), idx.reshape(fgw.shape)
-        f = np.asarray(fgw, dtype=np.float64)
-        best, idx = self._run_verified(lists, lambda pack: pack.fe_skymax(f.reshape(-1), fplus, fcross),
-                                       asynchronous=False)
-        if f.ndim == 0:
+        best, idx = self._run_verified((Nvecs, Ts, sigmas), run, asynchronous=on_device)
+        if not on_device and np.ndim(fgw) == 0:
             return float(best[0]), int(idx[0])
-        return best.reshape(f.shape), idx.reshape(f.shape)
+        return best.reshape(np.shape(fgw)), idx.reshape(np.shape(fgw))
 
     def calculate_Fe_skymax_batch(self, fgw, gwtheta, gwphi, Nvecs, Ts, sigmas, residuals):
         """:meth:`calculate_Fe_skymax` for each of ``R`` realisations of the residuals, with the pulsars, noise model
@@ -113,33 +90,17 @@ class FastFe(FastFp):
         DESIGN.md section 5e). One sky position is a targeted search at a known position."""
         fplus, fcross = self._sky_grid(gwtheta, gwphi)
         R, passes = self._residual_passes(residuals)
-        lists = (Nvecs, Ts, sigmas)
-        if _is_cuda_tensor(fgw):
-            import torch
-
-            f, stream = self._device_freqs(fgw)
-            best = torch.empty((R, f.shape[0]), dtype=torch.float64, device=f.device)
-            idx = torch.empty((R, f.shape[0]), dtype=torch.int64, device=f.device)
-
-            def run(pack):
-                for lo, _ in passes(pack, stream):
-                    pack.fe_skymax_residuals((f.data_ptr(), f.shape[0]), fplus, fcross, out=best[lo].data_ptr(),
-                                             index_out=idx[lo].data_ptr(), stream=stream)
-                return best, idx
-
-            best, idx = self._run_verified(lists, run, asynchronous=True)
-            return best.reshape((R,) + tuple(fgw.shape)), idx.reshape((R,) + tuple(fgw.shape))
-        f = np.asarray(fgw, dtype=np.float64)
-        fl = f.reshape(-1)
+        f, empty, stream, on_device = self._front_end(fgw)
+        best, idx = empty((R, f.shape[0])), empty((R, f.shape[0]), np.int64)
 
         def run(pack):
-            best, idx = np.empty((R, fl.shape[0])), np.empty((R, fl.shape[0]), dtype=np.int64)
-            for lo, hi in passes(pack):
-                pack.fe_skymax_residuals(fl, fplus, fcross, out=best[lo:hi], index_out=idx[lo:hi])
+            for lo, hi in passes(pack, stream):
+                pack.fe_skymax_residuals(f, fplus, fcross, out=best[lo:hi], index_out=idx[lo:hi], stream=stream)
             return best, idx
 
-        best, idx = self._run_verified(lists, run, asynchronous=False)
-        return best.reshape((R,) + f.shape), idx.reshape((R,) + f.shape)
+        best, idx = self._run_verified((Nvecs, Ts, sigmas), run, asynchronous=on_device)
+        shape = (R,) + np.shape(fgw)
+        return best.reshape(shape), idx.reshape(shape)
 
     def _sky_grid(self, gwtheta, gwphi):
         """Antenna patterns ``(F+, Fx)``, each ``(S, P)``, of the sky grid ``gwtheta``, ``gwphi`` broadcast to ``(S,)``."""

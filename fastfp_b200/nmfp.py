@@ -21,7 +21,8 @@ from __future__ import annotations
 import numpy as np
 
 from . import constants as const
-from .fastfp import _PackCache, _is_cuda_tensor
+from ._cabi import _is_cuda_tensor
+from .fastfp import _PackCache
 
 
 def _powerlaw(Ffreqs, log10_A, gamma):
