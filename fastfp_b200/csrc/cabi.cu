@@ -807,13 +807,13 @@ int fastfp_tnt(int device, int64_t n, int64_t m, const double* Nvec, const doubl
 }
 
 int fastfp_fp64_peak(int device, int kind, int iters, double* tflops, double* ms) {
-  if (!tflops || !ms || iters < 1 || kind < 0 || kind > 18) {
+  if (!tflops || !ms || iters < 1 || kind < 0 || kind > 24) {
     set_error("fastfp_fp64_peak: invalid argument");
     return FASTFP_ERR_INVALID;
   }
   DeviceGuard g(device);
   if (!g.ok) { set_error("cannot select CUDA device"); return FASTFP_ERR_CUDA; }
-  if (kind >= 17) return run_i8_peak(kind, iters, tflops, ms);
+  if (kind == 17 || kind == 18) return run_i8_peak(kind, iters, tflops, ms);
   return run_fp64_peak(kind, iters, tflops, ms);
 }
 

@@ -23,9 +23,9 @@ constexpr int VST = 16;        // TOA-vector ring depth (t | 1/N | w; TMA -> pro
 constexpr int FLUSH_TOAS = 512;  // level-1 accumulation block, in TOAs
 constexpr int MAX_M = 640;     // widest basis the sweep kernel handles (8 warp rows x 10 blocks of 8 rows)
 
-// Sweep configuration. The contraction runs on the fp64 MMA path (mma.sync.m8n8k4.f64): a warp
-// owns NMBW row blocks (8 basis rows each) x NNB column blocks (8 columns = 4 frequencies x
-// {sin, cos}); WMW consumer warps split the rows, NWC/WMW split the frequencies of the tile.
+// Sweep configuration. The contraction runs on the fp64 MMA path (mma.sync.m16n8k4.f64, basis rows on the N side): a
+// warp owns NMBW row blocks (8 basis rows each) x NNB/2 tiles of 8 frequencies x {sin, cos} (the 16 MMA rows), i.e.
+// 4*NNB frequencies; WMW consumer warps split the rows, NWC/WMW split the frequencies of the tile.
 //   CI  TOAs per staged chunk (KB = CI/4 k-blocks)
 //   NWC / NWP  consumer (MMA) / producer (sincos) warps of the CTA. The MMA issue rate of one warp is
 //   limited, so narrow accumulator tiles want three consumer warps per SM sub-partition (12 + 8);
@@ -40,11 +40,10 @@ struct SweepCfg {
   static_assert(NTC * CREGS + NTP * PREGS <= NTHREADS * ((65536 / NTHREADS) / 8 * 8), "register pool");
   static constexpr int WNW = NWC / WMW;        // consumer warps along frequency
   static constexpr int KF = WNW * NNB * 4;     // frequencies per CTA
-  static constexpr int NBT = KF / 4;           // column blocks per CTA tile
   static constexpr int NMB = NMBW * WMW;       // row blocks
   static constexpr int MP = 8 * NMB;           // padded basis width (rows of G)
   static constexpr int KB = CI / 4;            // k-blocks (4 TOAs) per chunk
-  static constexpr int ST = CI * 2 * KF;       // doubles of one sin/cos tile: [KB][NBT][32]
+  static constexpr int ST = CI * 2 * KF;       // doubles of one sin/cos tile: [KB][NX][32][2]
   static constexpr int VEC = 4 * CI;           // doubles of the vector part: (t, 1/N, w, 0) per TOA
   static constexpr int GT = CI * MP;           // doubles of the G part: [KB][NMB][32] fragments
   static constexpr int PK = VEC + GT;          // doubles per packet
@@ -73,8 +72,8 @@ struct SweepCfg {
 };
 
 // offset of G element (TOA il within its chunk, basis row j) inside a packet's G part:
-// fragment order [k-block][row block][lane], lane = (j%8)*4 + il%4 -- the A-operand layout of
-// mma.m8n8k4 (row = lane>>2, k = lane&3), so a warp's fragment load is 256 contiguous bytes.
+// fragment order [k-block][row block][lane], lane = (j%8)*4 + il%4 -- the B-operand layout of
+// mma.m16n8k4 (n = lane>>2, k = lane&3), so a warp's fragment load is 256 contiguous bytes.
 __host__ __device__ inline int g_frag_index(int il, int j, int nmb) {
   return (((il >> 2) * nmb + (j >> 3)) << 5) + (((j & 7) << 2) | (il & 3));
 }

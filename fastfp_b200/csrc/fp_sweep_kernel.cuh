@@ -12,9 +12,9 @@
 //     producers  : build sin/cos of ((2*pi)*f)*t (fastfp.py:78-79 phase order, one rounding per
 //                  multiply) for their (frequency, TOA) pairs, store them into the shared S-tile
 //                  ring in MMA-fragment order, and accumulate s N^-1 s, s N^-1 c, c N^-1 c, s.w, c.w
-//     consumers  : Y[MP][2*KF] += G_chunk^T . S_chunk on the fp64 MMA path (mma.sync.m8n8k4.f64;
-//                  measured to share the DFMA pipe and its peak, but with one 8-byte operand load
-//                  per 128 FMAs instead of one per ~4)
+//     consumers  : Y^T[2*KF][MP] += S_chunk^T . G_chunk on the fp64 MMA path (mma.sync.m16n8k4.f64: 16 rows =
+//                  8 frequencies x {sin, cos}, 8 columns = basis rows, k = TOAs; it shares the pipe with DFMA
+//                  but runs at twice m8n8k4's rate on H100, DESIGN.md section 4.1)
 //   epilogue     : b = Y_s.Y_s, Y_s.Y_c, Y_c.Y_c; M = [[sNs-b_ss, sNc-b_sc],[.., cNc-b_cc]],
 //                  N = [s.w, c.w]; general 2x2 solve with partial pivoting (what jnp.linalg.solve
 //                  does at fastfp.py:90); term = 0.5 * N . M^-1 N.
@@ -69,11 +69,12 @@ struct SweepArgs {
 #define FFP_DBG(ar, bit) 0
 #endif
 
-// D(8x8) += A(8x4) . B(4x8), fp64. Lane l holds A[l>>2][l&3], B[l&3][l>>2], D[l>>2][2*(l&3)+{0,1}].
-__device__ __forceinline__ void dmma_m8n8k4(double& d0, double& d1, double a, double b) {
-  asm("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-      : "+d"(d0), "+d"(d1)
-      : "d"(a), "d"(b));
+// D(16x8) += A(16x4) . B(4x8), fp64. With g = l>>2, t = l&3, lane l holds A[g][t], A[g+8][t] (a0, a1), B[t][g] (b),
+// D[g][2t+{0,1}] (d0, d1) and D[g+8][2t+{0,1}] (d2, d3).
+__device__ __forceinline__ void dmma_m16n8k4(double (&d)[4], double a0, double a1, double b) {
+  asm("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+      : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
+      : "d"(a0), "d"(a1), "d"(b));
 }
 template <int R>
 __device__ __forceinline__ void reg_alloc() {
@@ -86,8 +87,8 @@ __device__ __forceinline__ void reg_dealloc() {
 // Shared-memory carve-up, identical for both roles.
 template <class C>
 struct SweepSmem {
-  double* Sring;   // [C::SST][KB][NBT][32]   sin/cos tiles, B-fragment order
-  double* Gring;   // [GST][KB][NMB][32]   G tiles, A-fragment order
+  double* Sring;   // [C::SST][KB][NX][32][2]  sin/cos tiles, A-fragment order (one (sin, cos) pair per lane)
+  double* Gring;   // [GST][KB][NMB][32]      G tiles, B-fragment order
   double* Vring;   // [VST][VEC]           t | 1/N | w
   double* fq;      // [KF]                 trial frequencies of the current tile
   double* red;     // [RED]                epilogue reduction scratch
@@ -122,9 +123,10 @@ __device__ __forceinline__ void producer_loop(const SweepArgs& ar, SweepSmem<C>&
   const int bx0 = C::NX >= C::NWP ? pw * XW : pw % C::NX;         // first group of 8 frequencies
   const int bkb0 = C::NX >= C::NWP ? 0 : (pw / C::NX) * C::KBW;   // first k-block
   const int bsplit = C::NX >= C::NWP ? 0 : pw / C::NX;
-  // element (frequency group x, k-block kb) -> S offset (kb*NBT + 2*x + (bf8>>2))*32 + 8*(bf8&3) + 2*bk:
-  // the (sin, cos) pair of a (TOA, frequency) is adjacent, so it goes out as one 16-byte store
-  const int sofs = (bf8 >> 2) * 32 + 8 * (bf8 & 3) + 2 * bk;
+  // element (frequency group x, k-block kb) -> S offset (kb*NX + x)*64 + 2*lane: the (sin, cos) pair of a (TOA,
+  // frequency) is the (a0, a1) fragment of the consumer lane with the same (frequency, TOA) -- one 16-byte store,
+  // 512 contiguous bytes per warp
+  const int sofs = 2 * lane;
   double* const sl = ar.slab + (size_t)blockIdx.x * C::SLAB + (size_t)C::NACCX * C::NTC + tidp;
   uint32_t g = 0;
   for (;;) {
@@ -184,7 +186,7 @@ __device__ __forceinline__ void producer_loop(const SweepArgs& ar, SweepSmem<C>&
               const double ph = __dmul_rn(omega[xx], tn.x);  // ((2*pi)*f)*t, rounded once more
               double s, cs;
               sincos_cw(ph, &s, &cs);
-              *reinterpret_cast<double2*>(sb + (kb * C::NBT + 2 * (bx0 + xx)) * 32) = make_double2(s, cs);
+              *reinterpret_cast<double2*>(sb + (kb * C::NX + bx0 + xx) * 64) = make_double2(s, cs);
               const double sn = s * tn.y, cn = cs * tn.y;
               s2[xx][0] = fma(sn, s, s2[xx][0]);
               s2[xx][1] = fma(sn, cs, s2[xx][1]);
@@ -204,7 +206,7 @@ __device__ __forceinline__ void producer_loop(const SweepArgs& ar, SweepSmem<C>&
             double s, cs;
             sincos(ph, &s, &cs);
             const double ni = pk[4 * i + 1], wv = pk[4 * i + 2];
-            *reinterpret_cast<double2*>(sb + (kb * C::NBT + 2 * (bx0 + xx)) * 32) = make_double2(s, cs);
+            *reinterpret_cast<double2*>(sb + (kb * C::NX + bx0 + xx) * 64) = make_double2(s, cs);
             const double sn = s * ni, cn = cs * ni;
 #pragma unroll
             for (int x2 = 0; x2 < XW; ++x2)
@@ -268,11 +270,12 @@ __device__ __forceinline__ void producer_loop(const SweepArgs& ar, SweepSmem<C>&
 template <class C, bool NMFP, bool ECORR, bool RES>
 __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>& sm, volatile int* s_work,
                                               const int cw, const int lane) {
-  constexpr int NMBW = C::NMBW, NNB = C::NNB;
+  // a warp owns NMBW blocks of 8 basis rows (the N side, B = G^T) x NMT tiles of 8 frequencies x {sin, cos} (the M
+  // side, A = S^T): lane (g, t) = (lane>>2, lane&3) loads sin and cos of (frequency g, TOA t) as one 16-byte pair
+  constexpr int NMBW = C::NMBW, NMT = C::NNB / 2;
+  static_assert(C::NNB % 2 == 0, "16-row MMA tiles: frequencies in groups of 8");
   const int tid = cw * 32 + lane;
   const int wm = cw / C::WNW, wn = cw - wm * C::WNW;
-  // B fragment: lane holds S[k = lane&3][n = lane>>2], n = 2*(freq%4) + {sin, cos}; stored at 8*(n>>1) + 2*k + (n&1)
-  const int bperm = 8 * (lane >> 3) + 2 * (lane & 3) + ((lane >> 2) & 1);
   double* const sl = ar.slab + (size_t)blockIdx.x * C::SLAB + tid;
   uint32_t g = 0;
   for (;;) {
@@ -299,33 +302,38 @@ __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>&
     if (tid < C::KF) sm.fq[tid] = ar.freqs[f0 + tid < ar.F ? f0 + tid : f0];
     __syncthreads();  // B2
 
-    double acc[NMBW][NNB][2];
+    // acc[r][q]: Y_sin of frequency 8*(wn*NMT + q) + g for basis rows 8*(wm*NMBW + r) + 2t + {0, 1}, then Y_cos
+    double acc[NMBW][NMT][4];
 #pragma unroll
     for (int r = 0; r < NMBW; ++r)
 #pragma unroll
-      for (int q = 0; q < NNB; ++q) acc[r][q][0] = acc[r][q][1] = 0.0;
+      for (int q = 0; q < NMT; ++q) acc[r][q][0] = acc[r][q][1] = acc[r][q][2] = acc[r][q][3] = 0.0;
     bool flushed = false;
-    // block-diagonal N (kernel ECORR): the last row block of the last warp row holds 8 epoch slots;
-    // Y there is sqrt(beta_e) * sum_{i in e} x_i / N_i, folded into these sums when the epoch ends
-    double es[NNB][3];
+    // block-diagonal N (kernel ECORR): the last row block of the last warp row holds 8 epoch slots (this thread:
+    // slots 2t, 2t+1, kept apart); Y there is sqrt(beta_e) * sum_{i in e} x_i / N_i, folded into these sums when the
+    // epoch ends
+    double es[NMT][2][3];
 #pragma unroll
-    for (int q = 0; q < NNB; ++q) es[q][0] = es[q][1] = es[q][2] = 0.0;
+    for (int q = 0; q < NMT; ++q)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) es[q][e][0] = es[q][e][1] = es[q][e][2] = 0.0;
     const bool slot_warp = ECORR && wm == C::WMW - 1;
     const unsigned char* dmask = ECORR ? ar.done_mask + pm.dm_off : nullptr;
 
     // fragments of the next k-block -- also across chunk boundaries -- are fetched while the MMAs of
     // the current one run
-    double a0[NMBW], b0[NNB];
+    double2 a0[NMT];
+    double b0[NMBW];
     {
       const uint32_t k = g;
       mbar_wait_spin(&sm.g_full[k % C::GST], (k / C::GST) & 1u);
       mbar_wait_spin(&sm.s_full[k % C::SST], (k / C::SST) & 1u);
       const double* gt = sm.Gring + (k % C::GST) * C::GT + (wm * NMBW) * 32 + lane;
-      const double* sb = sm.Sring + (k % C::SST) * C::ST + (wn * NNB) * 32 + bperm;
+      const double* sb = sm.Sring + (k % C::SST) * C::ST + (wn * NMT) * 64 + 2 * lane;
 #pragma unroll
-      for (int r = 0; r < NMBW; ++r) a0[r] = gt[r * 32];
+      for (int r = 0; r < NMBW; ++r) b0[r] = gt[r * 32];
 #pragma unroll
-      for (int q = 0; q < NNB; ++q) b0[q] = sb[q * 32];
+      for (int q = 0; q < NMT; ++q) a0[q] = *reinterpret_cast<const double2*>(sb + q * 64);
     }
     for (int c = 0; c < nch; ++c) {
       const uint32_t k = g + (uint32_t)c;
@@ -335,41 +343,42 @@ __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>&
         issue_G(c + C::GST - 2);
       }
       const double* gt = sm.Gring + (k % C::GST) * C::GT + (wm * NMBW) * 32 + lane;
-      const double* sb = sm.Sring + (k % C::SST) * C::ST + (wn * NNB) * 32 + bperm;
+      const double* sb = sm.Sring + (k % C::SST) * C::ST + (wn * NMT) * 64 + 2 * lane;
 #pragma unroll
       for (int kb = 0; kb < C::KB; ++kb) {
-        double a1[NMBW], b1[NNB];
+        double2 a1[NMT];
+        double b1[NMBW];
         if (kb + 1 < C::KB) {
 #pragma unroll
-          for (int r = 0; r < NMBW; ++r) a1[r] = gt[((kb + 1) * C::NMB + r) * 32];
+          for (int r = 0; r < NMBW; ++r) b1[r] = gt[((kb + 1) * C::NMB + r) * 32];
 #pragma unroll
-          for (int q = 0; q < NNB; ++q) b1[q] = sb[((kb + 1) * C::NBT + q) * 32];
+          for (int q = 0; q < NMT; ++q) a1[q] = *reinterpret_cast<const double2*>(sb + ((kb + 1) * C::NX + q) * 64);
         } else if (c + 1 < nch) {
           const uint32_t k1 = k + 1;
           mbar_wait_spin(&sm.g_full[k1 % C::GST], (k1 / C::GST) & 1u);
           mbar_wait_spin(&sm.s_full[k1 % C::SST], (k1 / C::SST) & 1u);
           const double* gt1 = sm.Gring + (k1 % C::GST) * C::GT + (wm * NMBW) * 32 + lane;
-          const double* sb1 = sm.Sring + (k1 % C::SST) * C::ST + (wn * NNB) * 32 + bperm;
+          const double* sb1 = sm.Sring + (k1 % C::SST) * C::ST + (wn * NMT) * 64 + 2 * lane;
 #pragma unroll
-          for (int r = 0; r < NMBW; ++r) a1[r] = gt1[r * 32];
+          for (int r = 0; r < NMBW; ++r) b1[r] = gt1[r * 32];
 #pragma unroll
-          for (int q = 0; q < NNB; ++q) b1[q] = sb1[q * 32];
+          for (int q = 0; q < NMT; ++q) a1[q] = *reinterpret_cast<const double2*>(sb1 + q * 64);
         } else {
 #pragma unroll
-          for (int r = 0; r < NMBW; ++r) a1[r] = 0.0;
+          for (int r = 0; r < NMBW; ++r) b1[r] = 0.0;
 #pragma unroll
-          for (int q = 0; q < NNB; ++q) b1[q] = 0.0;
+          for (int q = 0; q < NMT; ++q) a1[q] = make_double2(0.0, 0.0);
         }
         if (!FFP_DBG(ar, 2)) {
 #pragma unroll
           for (int r = 0; r < NMBW; ++r)
 #pragma unroll
-            for (int q = 0; q < NNB; ++q) dmma_m8n8k4(acc[r][q][0], acc[r][q][1], a0[r], b0[q]);
+            for (int q = 0; q < NMT; ++q) dmma_m16n8k4(acc[r][q], a0[q].x, a0[q].y, b0[r]);
         }
 #pragma unroll
-        for (int r = 0; r < NMBW; ++r) a0[r] = a1[r];
+        for (int r = 0; r < NMBW; ++r) b0[r] = b1[r];
 #pragma unroll
-        for (int q = 0; q < NNB; ++q) b0[q] = b1[q];
+        for (int q = 0; q < NMT; ++q) a0[q] = a1[q];
       }
       __syncwarp();
       if (lane == 0) {
@@ -378,43 +387,46 @@ __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>&
       }
       if (ECORR && slot_warp) {
         // epochs that end in this chunk: e_xy += (sqrt(beta) A_x)(sqrt(beta) A_y); the slot restarts
-        if ((dmask[c] >> (lane >> 2)) & 1) {
+        const unsigned dm = (unsigned)dmask[c] >> (2 * (lane & 3));
 #pragma unroll
-          for (int q = 0; q < NNB; ++q) {
-            const double ys = acc[NMBW - 1][q][0], yc = acc[NMBW - 1][q][1];
-            es[q][0] = fma(ys, ys, es[q][0]);
-            es[q][1] = fma(ys, yc, es[q][1]);
-            es[q][2] = fma(yc, yc, es[q][2]);
-            acc[NMBW - 1][q][0] = acc[NMBW - 1][q][1] = 0.0;
+        for (int e = 0; e < 2; ++e)
+          if ((dm >> e) & 1u) {
+#pragma unroll
+            for (int q = 0; q < NMT; ++q) {
+              const double ys = acc[NMBW - 1][q][e], yc = acc[NMBW - 1][q][2 + e];
+              es[q][e][0] = fma(ys, ys, es[q][e][0]);
+              es[q][e][1] = fma(ys, yc, es[q][e][1]);
+              es[q][e][2] = fma(yc, yc, es[q][e][2]);
+              acc[NMBW - 1][q][e] = acc[NMBW - 1][q][2 + e] = 0.0;
+            }
           }
-        }
       }
       if ((c + 1) % C::FLUSH == 0 && c + 1 < nch && !FFP_DBG(ar, 4)) {
         // fold the level-1 sums into the level-2 totals of this CTA's scratch slab
 #pragma unroll
         for (int r = 0; r < NMBW; ++r)
 #pragma unroll
-          for (int q = 0; q < NNB; ++q)
+          for (int q = 0; q < NMT; ++q)
 #pragma unroll
-            for (int e = 0; e < 2; ++e) {
+            for (int e = 0; e < 4; ++e) {
               if (ECORR && r == NMBW - 1 && slot_warp) continue;  // open epoch sums stay in registers
               // the slot is private to this thread: first block stores, later blocks add with a
               // fire-and-forget reduction (RED.ADD.F64) -- a load/add/store chain would expose one L2
               // round trip per accumulator
-              double* a = sl + (size_t)((r * NNB + q) * 2 + e) * C::NTC;
+              double* a = sl + (size_t)((r * NMT + q) * 4 + e) * C::NTC;
               if (flushed) atomicAdd(a, acc[r][q][e]);
               else __stcg(a, acc[r][q][e]);
               acc[r][q][e] = 0.0;
             }
         if (ECORR && slot_warp) {
 #pragma unroll
-          for (int q = 0; q < NNB; ++q)
+          for (int q = 0; q < NMT; ++q)
 #pragma unroll
-            for (int e = 0; e < 3; ++e) {
-              double* a = sl + (size_t)(C::NACC + q * 3 + e) * C::NTC;
-              if (flushed) atomicAdd(a, es[q][e]);
-              else __stcg(a, es[q][e]);
-              es[q][e] = 0.0;
+            for (int e = 0; e < 6; ++e) {
+              double* a = sl + (size_t)(C::NACC + q * 6 + e) * C::NTC;
+              if (flushed) atomicAdd(a, es[q][e / 3][e % 3]);
+              else __stcg(a, es[q][e / 3][e % 3]);
+              es[q][e / 3][e % 3] = 0.0;
             }
         }
         flushed = true;
@@ -428,35 +440,40 @@ __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>&
 #pragma unroll
       for (int r = 0; r < NMBW; ++r)
 #pragma unroll
-        for (int q = 0; q < NNB; ++q)
+        for (int q = 0; q < NMT; ++q)
 #pragma unroll
-          for (int e = 0; e < 2; ++e)
-            if (!(ECORR && r == NMBW - 1 && slot_warp)) acc[r][q][e] += __ldcg(sl + (size_t)((r * NNB + q) * 2 + e) * C::NTC);
+          for (int e = 0; e < 4; ++e)
+            if (!(ECORR && r == NMBW - 1 && slot_warp)) acc[r][q][e] += __ldcg(sl + (size_t)((r * NMT + q) * 4 + e) * C::NTC);
       if (ECORR && slot_warp) {
 #pragma unroll
-        for (int q = 0; q < NNB; ++q)
+        for (int q = 0; q < NMT; ++q)
 #pragma unroll
-          for (int e = 0; e < 3; ++e) es[q][e] += __ldcg(sl + (size_t)(C::NACC + q * 3 + e) * C::NTC);
+          for (int e = 0; e < 6; ++e) es[q][e / 3][e % 3] += __ldcg(sl + (size_t)(C::NACC + q * 6 + e) * C::NTC);
       }
     }
-    // this thread holds Y[row][freq] for rows 8*(wm*NMBW + r) + (lane>>2) and the tile frequencies
-    // 4*(wn*NNB + q) + (lane&3): [..][0] is the sin column, [..][1] the cos column
+    // this thread holds Y of the tile frequency 8*(wn*NMT + q) + (lane>>2) for the rows 8*(wm*NMBW + r) +
+    // 2*(lane&3) + e: acc[r][q][e] is the sin column, acc[r][q][2 + e] the cos column
+    // b-sums: one fma chain per row residue j%8 over the warp's row blocks, then a pairwise tree over the 8 residues --
+    // (2t, 2t+1) in registers, then the t-lanes -- so a frequency's sums are rounded the same way whatever the MMA
+    // shape and the lane that owns a row
     const int mfix = pm.mfix;  // rows below mfix enter the b-sums (plain Fp: mfix = m)
     double* redB = sm.red;  // [WMW][KF][3]
 #pragma unroll
-    for (int q = 0; q < NNB; ++q) {
-      double pss = 0, psc = 0, pcc = 0;
+    for (int q = 0; q < NMT; ++q) {
+      double ps[2][3] = {{0, 0, 0}, {0, 0, 0}};  // (ss, sc, cc) of rows 2t, 2t+1 mod 8
 #pragma unroll
-      for (int r = 0; r < NMBW; ++r) {
-        const int j = 8 * (wm * NMBW + r) + (lane >> 2);
-        const double ys = acc[r][q][0], yc = acc[r][q][1];
+      for (int r = 0; r < NMBW; ++r)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int j = 8 * (wm * NMBW + r) + 2 * (lane & 3) + e;
+        const double ys = acc[r][q][e], yc = acc[r][q][2 + e];
         if (j < mfix) {
-          pss = fma(ys, ys, pss);
-          psc = fma(ys, yc, psc);
-          pcc = fma(yc, yc, pcc);
+          ps[e][0] = fma(ys, ys, ps[e][0]);
+          ps[e][1] = fma(ys, yc, ps[e][1]);
+          ps[e][2] = fma(yc, yc, ps[e][2]);
         } else if (NMFP && j < pm.m) {
           // nmfp: rows of the per-draw block go out as z' (canonical 32-frequency tiles)
-          const int64_t f = f0 + 4 * (wn * NNB + q) + (lane & 3);
+          const int64_t f = f0 + 8 * (wn * NMT + q) + (lane >> 2);
           if (f < ar.F) {
             // 32-frequency tile, MMA B-fragment order: k-block (row/4), column block (4 freqs), then
             // position 16*sc + 4*(freq%4) + row%4 -- the layout stage B loads without conflicts
@@ -469,19 +486,16 @@ __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>&
           }
         }
       }
-      if (ECORR && slot_warp) {  // the block-N correction enters exactly like the Woodbury b-sums
-        pss += es[q][0];
-        psc += es[q][1];
-        pcc += es[q][2];
-      }
-      double v3[3] = {pss, psc, pcc};
 #pragma unroll
       for (int k = 0; k < 3; ++k) {
-        double v = v3[k];
-        v += __shfl_xor_sync(0xffffffffu, v, 4);
-        v += __shfl_xor_sync(0xffffffffu, v, 8);
-        v += __shfl_xor_sync(0xffffffffu, v, 16);
-        if ((lane >> 2) == 0) redB[(wm * C::KF + 4 * (wn * NNB + q) + (lane & 3)) * 3 + k] = v;
+        if (ECORR && slot_warp) {  // the block-N correction enters exactly like the Woodbury b-sums, per slot
+          ps[0][k] += es[q][0][k];
+          ps[1][k] += es[q][1][k];
+        }
+        double v = ps[0][k] + ps[1][k];
+        v += __shfl_xor_sync(0xffffffffu, v, 1);
+        v += __shfl_xor_sync(0xffffffffu, v, 2);
+        if ((lane & 3) == 0) redB[(wm * C::KF + 8 * (wn * NMT + q) + (lane >> 2)) * 3 + k] = v;
       }
     }
     __syncthreads();  // B3: reductions (consumer b-sums, producer scalar sums) published
@@ -535,23 +549,25 @@ __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>&
       asm volatile("bar.sync 1, %0;" ::"n"(C::NTC) : "memory");  // consumers only: M of every frequency is published
       const int r0 = (pm.m + 7) & ~7;
 #pragma unroll
-      for (int q = 0; q < NNB; ++q) {
-        const int fl = 4 * (wn * NNB + q) + (lane & 3);
+      for (int q = 0; q < NMT; ++q) {
+        const int fl = 8 * (wn * NMT + q) + (lane >> 2);
         const int64_t f = f0 + fl;
         if (f >= ar.F) continue;
         const double m00 = redB[fl * 3], m01 = redB[fl * 3 + 1], m11 = redB[fl * 3 + 2];
         const bool fpos = sm.fq[fl] > 0.0;
 #pragma unroll
-        for (int r = 0; r < NMBW; ++r) {
-          const int k = 8 * (wm * NMBW + r) + (lane >> 2) - r0;
+        for (int r = 0; r < NMBW; ++r)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int k = 8 * (wm * NMBW + r) + 2 * (lane & 3) + e - r0;
           if (k < 0 || k >= ar.nres) continue;
           if (ar.inner) {  // inner-product output: (s|r_k), (c|r_k) as [F][P][R][2]
             const double nan = __longlong_as_double(0x7ff8000000000000LL);
             *reinterpret_cast<double2*>(ar.terms + (((size_t)f * ar.npsr + p) * ar.nres + k) * 2) =
-                fpos ? make_double2(acc[r][q][0], acc[r][q][1]) : make_double2(nan, nan);
+                fpos ? make_double2(acc[r][q][e], acc[r][q][2 + e]) : make_double2(nan, nan);
             continue;
           }
-          double val = term_2x2(m00, m01, m11, acc[r][q][0], acc[r][q][1]);
+          double val = term_2x2(m00, m01, m11, acc[r][q][e], acc[r][q][2 + e]);
           if (!fpos) val = __longlong_as_double(0x7ff8000000000000LL);
           ar.terms[((size_t)k * ar.npsr + p) * ar.F + f] = val;
         }

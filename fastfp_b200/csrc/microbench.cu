@@ -1,5 +1,6 @@
 // fp64 pipe peak: the measured denominator for the sweep kernel's fp64 roofline
-// (MEASURED_PEAKS.json carries only HBM and bf16 figures). kind 0 = DFMA, kind 1 = DMMA m8n8k4.
+// (MEASURED_PEAKS.json carries only HBM and bf16 figures). kind 0 = DFMA, kind 1 = DMMA m16n8k4 (the shape the
+// sweep kernel issues), kind 19 = DMMA m8n8k4.
 #include "ffp_internal.cuh"
 #include "ffp_sincos.cuh"
 
@@ -285,6 +286,118 @@ __global__ void __launch_bounds__(256) imma_peak_kernel(int iters, int seed, dou
   if (s == 123456789) sink[0] = (double)s;
 }
 
+// kinds 1, 20, 21: the 16x8 fp64 MMA shapes m16n8k{4,8,16} (sm_90+), 8 independent accumulators per warp and four
+// warps per SM sub-partition, so that the MMA latency is hidden and only the issue rate of the shape remains
+template <int K>
+__device__ __forceinline__ void dmma_m16n8(double (&c)[4], const double (&a)[K / 2], const double (&b)[K / 4]) {
+  if constexpr (K == 4)
+    asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+                 : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+                 : "d"(a[0]), "d"(a[1]), "d"(b[0]));
+  else if constexpr (K == 8)
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, "
+                 "{%0,%1,%2,%3};"
+                 : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+                 : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
+  else
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, "
+                 "{%4,%5,%6,%7,%8,%9,%10,%11}, {%12,%13,%14,%15}, {%0,%1,%2,%3};"
+                 : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+                 : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]), "d"(b[0]),
+                   "d"(b[1]), "d"(b[2]), "d"(b[3]));
+}
+
+template <int K>
+__global__ void __launch_bounds__(256, 2) dmma16_peak_kernel(int iters, double seed, double* sink) {
+  double c[8][4];
+#pragma unroll
+  for (int k = 0; k < 8; ++k)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) c[k][j] = seed + k + j;
+  double a[K / 2], b[K / 4];
+#pragma unroll
+  for (int k = 0; k < K / 2; ++k) a[k] = 1.0 + (threadIdx.x + k) * 1e-9;
+#pragma unroll
+  for (int k = 0; k < K / 4; ++k) b[k] = 1e-3 * (k + 1);
+  for (int it = 0; it < iters; ++it) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) dmma_m16n8<K>(c[k], a, b);
+  }
+  double s = 0;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) s += c[k][0] + c[k][1] + c[k][2] + c[k][3];
+  if (s == 12345.678) sink[0] = s;
+}
+
+// kind 22: kinds 13-15's warp specialisation with the sweep's m16n8k4 -- 8 warps issue m16n8k4 (8 accumulators each),
+// 16 warps issue DFMA chains, with as many DFMAs per MMA FMA as kind 14 (the sweep kernel's producer ratio)
+__global__ void __launch_bounds__(768, 1) warp_mix16_kernel(int iters, double seed, double* sink) {
+  const int w = threadIdx.x >> 5;
+  double s = 0;
+  if (w < 8) {
+    double c[8][4];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) c[k][0] = c[k][1] = c[k][2] = c[k][3] = seed + k;
+    const double a[2] = {1.0 + threadIdx.x * 1e-9, 1.0}, b[1] = {1e-3};
+    for (int it = 0; it < iters; ++it) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) dmma_m16n8<4>(c[k], a, b);
+    }
+#pragma unroll
+    for (int k = 0; k < 8; ++k) s += c[k][0] + c[k][1] + c[k][2] + c[k][3];
+  } else {
+    // twice kind 14's DFMA iterations: a DMMA warp iteration here is 8 x 512 FMAs, there 8 x 256
+    const int itf = (int)((long long)iters * 4 * 50 / 256);
+    double a[16];
+#pragma unroll
+    for (int k = 0; k < 16; ++k) a[k] = seed + k + threadIdx.x * 1e-3;
+    const double x = 1.0000001, y = 1e-9;
+    for (int it = 0; it < itf; ++it) {
+#pragma unroll
+      for (int k = 0; k < 16; ++k) a[k] = fma(a[k], x, y);
+    }
+#pragma unroll
+    for (int k = 0; k < 16; ++k) s += a[k];
+  }
+  if (s == 12345.678) sink[0] = s;
+}
+
+// kinds 23, 24: the consumer's pattern with the 16x8 shapes -- NMBW basis-row blocks (B operand, one 256-byte warp
+// load per k-block each) x one 16-row tile of 8 frequencies x {sin, cos} (A operand, one 128-bit load per lane and
+// k-block), fragments re-read from shared memory for every k-step, two warps per SM sub-partition
+template <int NMBW, int K>
+__global__ void __launch_bounds__(256) dmma16_tile_kernel(int iters, double seed, double* sink) {
+  constexpr int KB = K / 4;  // k-blocks of 4 per MMA
+  __shared__ double sh[2 * KB * (NMBW + 2) * 32];
+  for (int i = threadIdx.x; i < 2 * KB * (NMBW + 2) * 32; i += blockDim.x) sh[i] = seed * 1e-3 + i * 1e-9;
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  double acc[NMBW][4];
+#pragma unroll
+  for (int r = 0; r < NMBW; ++r) acc[r][0] = acc[r][1] = acc[r][2] = acc[r][3] = seed;
+  for (int it = 0; it < iters; ++it) {
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks) {
+      const volatile double* va = sh + ks * KB * (NMBW + 2) * 32;
+      double a[K / 2], b[NMBW][K / 4];
+#pragma unroll
+      for (int kb = 0; kb < KB; ++kb) {
+        asm volatile("ld.volatile.shared.v2.f64 {%0, %1}, [%2];"
+                     : "=d"(a[2 * kb]), "=d"(a[2 * kb + 1])
+                     : "r"(smem_u32((const void*)(va + (kb * (NMBW + 2) + NMBW) * 32 + 2 * lane))));
+#pragma unroll
+        for (int r = 0; r < NMBW; ++r) b[r][kb] = va[(kb * (NMBW + 2) + r) * 32 + lane];
+      }
+#pragma unroll
+      for (int r = 0; r < NMBW; ++r) dmma_m16n8<K>(acc[r], a, b[r]);
+    }
+  }
+  double s = 0;
+#pragma unroll
+  for (int r = 0; r < NMBW; ++r) s += acc[r][0] + acc[r][1] + acc[r][2] + acc[r][3];
+  if (s == 12345.678) sink[0] = s;
+}
+
 int run_fp64_peak(int kind, int iters, double* tflops, double* ms_out) {
   int dev = 0, sms = 0;
   FFP_CUDA(cudaGetDevice(&dev));
@@ -321,7 +434,13 @@ int run_fp64_peak(int kind, int iters, double* tflops, double* ms_out) {
   for (int rep = 0; rep < 4; ++rep) {
     FFP_CUDA(cudaEventRecord(e0));
     if (kind == 0) dfma_peak_kernel<<<grid, 256>>>(iters, 1.0, sink);
-    else if (kind == 1) dmma_peak_kernel<<<grid, 256>>>(iters, 1.0, sink);
+    else if (kind == 19) dmma_peak_kernel<<<grid, 256>>>(iters, 1.0, sink);
+    else if (kind == 1) dmma16_peak_kernel<4><<<sms * 2, 256>>>(iters, 1.0, sink);    // 4 warps / sub-partition
+    else if (kind == 20) dmma16_peak_kernel<8><<<sms * 2, 256>>>(iters, 1.0, sink);
+    else if (kind == 21) dmma16_peak_kernel<16><<<sms * 2, 256>>>(iters, 1.0, sink);
+    else if (kind == 22) warp_mix16_kernel<<<sms, 768>>>(iters, 1.0, sink);
+    else if (kind == 23) dmma16_tile_kernel<9, 4><<<sms, 256>>>(iters, 1.0, sink);     // 2 warps / sub-partition
+    else if (kind == 24) dmma16_tile_kernel<9, 8><<<sms, 256>>>(iters, 1.0, sink);
     else if (kind == 2) mixed_peak_kernel<<<grid, 256>>>(iters, 1.0, sink);
     else if (kind == 9) dmma_tile_kernel<9, 2><<<sms, 256>>>(iters, 1.0, sink);    // 2 warps / sub-partition
     else if (kind == 10) dmma_tile_kernel<9, 2><<<sms, 512>>>(iters, 1.0, sink);   // 4 warps / sub-partition
@@ -341,9 +460,14 @@ int run_fp64_peak(int kind, int iters, double* tflops, double* ms_out) {
   }
   g_launches += 4;
   FFP_CUDA(cudaGetLastError());
-  // DFMA: 16 fma/thread/iter; DMMA: 8 mma/warp/iter, 8*8*4 fma each
+  // DFMA: 16 fma/thread/iter; DMMA: 8 mma/warp/iter, 8*8*4 fma each (16*8*K for the 16x8 shapes)
   const double fma_count = kind == 0   ? (double)grid * 256 * 16.0 * iters
-                           : kind == 1 ? (double)grid * 8 * 8.0 * 256.0 * iters
+                           : kind == 19 ? (double)grid * 8 * 8.0 * 256.0 * iters
+                           : kind == 1 || kind == 20 || kind == 21
+                               ? (double)sms * 16 * 8 * (128.0 * (kind == 1 ? 4 : kind == 20 ? 8 : 16)) * iters
+                           : kind == 22 ? (double)sms * (8 * 8 * 512.0 * iters +
+                                                         16 * 32 * 16.0 * (double)((long long)iters * 4 * 50 / 256))
+                           : kind == 23 || kind == 24 ? (double)sms * 8 * 2 * 9 * (128.0 * (kind == 23 ? 4 : 8)) * iters
                            : kind == 9 ? (double)sms * 8 * 2 * 18 * 256.0 * iters
                            : kind == 10 ? (double)sms * 16 * 2 * 18 * 256.0 * iters
                            : kind == 11 ? (double)sms * 4 * 2 * 36 * 256.0 * iters
