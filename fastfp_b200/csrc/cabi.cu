@@ -428,13 +428,13 @@ static int fp_run(const fastfp_pack* pk, const double* freqs, int64_t F, double*
   double* d_out;
   if (int rc = c.stage(freqs, F, out, nout, flags, &d_freqs, &d_out, want_terms ? &pk->terms : &pk->out)) return rc;
   if (want_terms) {
-    if (int rc = launch_sweep(pk, d_freqs, F, d_out, c.st)) return rc;
+    if (int rc = launch_sweep(pk, d_freqs, F, FpOut{d_out, nullptr}, c.st)) return rc;
   } else {
     const int64_t FB = freq_batch(F, P);
     if (int rc = pk->terms.grow((int64_t)P * std::min(FB, F))) return rc;
     for (int64_t lo = 0; lo < F; lo += FB) {
       const int64_t fb = std::min(FB, F - lo);
-      if (int rc = launch_sweep(pk, d_freqs + lo, fb, pk->terms.get(), c.st)) return rc;
+      if (int rc = launch_sweep(pk, d_freqs + lo, fb, FpOut{pk->terms.get(), nullptr}, c.st)) return rc;
       if (int rc = launch_reduce_terms(pk->terms.get(), P, fb, d_out + lo, c.st)) return rc;
     }
   }
@@ -512,7 +512,8 @@ int fastfp_fp_sweep_residuals(const fastfp_pack_t* pk, const double* freqs, int6
   if (int rc = pk->res_terms.grow(R * P * std::min(FB, F))) return rc;
   for (int64_t lo = 0; lo < F; lo += FB) {
     const int64_t fb = std::min(FB, F - lo);
-    if (int rc = launch_fp_sweep_res(pk, d_freqs + lo, fb, pk->res_terms.get(), c.st)) return rc;
+    const ResOut ro{pk->res_terms.get(), nullptr, nullptr, (int)R, P};
+    if (int rc = launch_fp_sweep_res(pk, d_freqs + lo, fb, ro, c.st)) return rc;
     if (int rc = launch_reduce_terms_rows(pk->res_terms.get(), (int)R, P, fb, d_out + lo, F, c.st)) return rc;
   }
   return c.finish(flags, R * F, out, d_out, false);
@@ -542,7 +543,7 @@ int fastfp_fe_sweep(const fastfp_pack_t* pk, const double* freqs, int64_t F, con
   if (int rc = c.upload_sky(fplus, fcross, S * P, d_fp, d_fx)) return rc;
   for (int64_t lo = 0; lo < F; lo += FB) {
     const int64_t fb = std::min(FB, F - lo);
-    if (int rc = launch_sweep(pk, d_freqs + lo, fb, nullptr, c.st, nullptr, d_inner)) return rc;
+    if (int rc = launch_sweep(pk, d_freqs + lo, fb, FpOut{nullptr, d_inner}, c.st)) return rc;
     if (int rc = launch_fe_combine(d_inner, P, fb, d_fp, d_fx, S, d_out + lo, F, c.st)) return rc;
   }
   return c.finish(flags, S * F, out, d_out, true);
@@ -588,7 +589,7 @@ int fastfp_fe_skymax(const fastfp_pack_t* pk, const double* freqs, int64_t F, co
   if (int rc = launch_fe_sky_weights(d_fp, d_fx, S * P, d_w, c.st)) return rc;
   for (int64_t lo = 0; lo < F; lo += FB) {
     const int64_t fb = std::min(FB, F - lo);
-    if (int rc = launch_sweep(pk, d_freqs + lo, fb, nullptr, c.st, nullptr, d_inner)) return rc;
+    if (int rc = launch_sweep(pk, d_freqs + lo, fb, FpOut{nullptr, d_inner}, c.st)) return rc;
     if (int rc = launch_fe_skymax(d_inner, P, fb, d_w, S, plan, part_v, part_i, d_max + lo, d_idx + lo, c.st))
       return rc;
   }
@@ -640,7 +641,8 @@ int fastfp_fe_skymax_residuals(const fastfp_pack_t* pk, const double* freqs, int
   if (int rc = c.upload_sky(fplus, fcross, S * P, d_fp, d_fx)) return rc;
   for (int64_t lo = 0; lo < F; lo += FB) {
     const int64_t fb = std::min(FB, F - lo);
-    if (int rc = launch_fp_sweep_res(pk, d_freqs + lo, fb, pk->res_terms.get(), c.st, d_mi)) return rc;
+    const ResOut ro{nullptr, pk->res_terms.get(), d_mi, (int)R, P};
+    if (int rc = launch_fp_sweep_res(pk, d_freqs + lo, fb, ro, c.st)) return rc;
     if (int rc = launch_fe_skymax_res(pk->res_terms.get(), d_mi, P, R, fb, d_fp, d_fx, S, plan, part_v, part_i,
                                       d_max + lo, d_idx + lo, F, c.st))
       return rc;

@@ -149,7 +149,7 @@ __global__ void __launch_bounds__(kSkyThreads, 3)
   const int64_t s_begin = (int64_t)blockIdx.y * chunk;
   const int64_t s_end = min(S, s_begin + chunk);
   const bool resident = P <= kSkyPC;
-  double best = __longlong_as_double(0x7ff8000000000000LL);
+  double best = kNaN();
   int64_t bidx = -1;
   for (int64_t s0 = s_begin; s0 < s_end; s0 += kSkyTile) {
     const int ns = s_end - s0 < kSkyTile ? (int)(s_end - s0) : kSkyTile;
@@ -246,13 +246,6 @@ constexpr int kResWS = 2 * kResSC + 4;       // pulsar stride of the pattern til
 constexpr int kResFac = 17;                  // doubles per factored M: 6 multipliers, 6 of U, 4 reciprocals, pivots
 constexpr size_t kResSmem = (size_t)(kResRows * kResPC * 2 + kResPC * kResWS + kResSC * 8 * kResFac) * sizeof(double);
 
-// D(8x8) += A(8x4) . B(4x8), fp64. Lane l holds A[l>>2][l&3], B[l&3][l>>2], D[l>>2][2*(l&3)+{0,1}].
-__device__ __forceinline__ void fe_dmma(double& d0, double& d1, double a, double b) {
-  asm("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-      : "+d"(d0), "+d"(d1)
-      : "d"(a), "d"(b));
-}
-
 // fe_solve's elimination on M alone: o = [l10 l20 l30 l21 l31 l32 | u01 u02 u03 u12 u13 u23 | 1/u00 .. 1/u33 | pivots]
 __device__ __forceinline__ void fe_factor(const double (&U)[4][4], double* o) {
   double M[4][4] = {{U[0][0], U[0][1], U[0][2], U[0][3]}, {U[0][1], U[1][1], U[1][2], U[1][3]},
@@ -332,7 +325,7 @@ __global__ void __launch_bounds__(kResThreads, 2)
   const int64_t s_begin = (int64_t)blockIdx.z * chunk;
   const int64_t s_end = min(S, s_begin + chunk);
   const bool resident = P <= kResPC;
-  const double nan = __longlong_as_double(0x7ff8000000000000LL);
+  const double nan = kNaN();
   // the M-stage thread of (frequency fl, sky position sl of the pass)
   const int m_fl = tid / kResSC, m_sl = tid % kResSC;
   const int64_t m_f = f0 + m_fl;
@@ -410,7 +403,7 @@ __global__ void __launch_bounds__(kResThreads, 2)
 #pragma unroll
           for (int ct = 0; ct < 4; ++ct)
 #pragma unroll
-            for (int sc = 0; sc < 2; ++sc) fe_dmma(acc[rt][ct][sc][0], acc[rt][ct][sc][1], a[rt][sc], b[ct]);
+            for (int sc = 0; sc < 2; ++sc) dmma_m8n8k4(acc[rt][ct][sc][0], acc[rt][ct][sc][1], a[rt][sc], b[ct]);
       }
     }
     __syncthreads();  // the factors of the pass are published

@@ -198,8 +198,8 @@ struct fastfp_pack {
   int mvar_max = 0;
   int mvpad = 0;           // nmfp: per-draw block width padded to the stage-B tile (32, 64 or 96)
   // nmfp only
-  double* d_S0 = nullptr;  // [P][mvmax][mvmax] Schur complement of the fixed block (no phiinv)
-  double* d_zr = nullptr;  // [P][mvmax]  z'_r
+  double* d_S0 = nullptr;  // [P][mvpad][mvpad] Schur complement of the fixed block (no phiinv)
+  double* d_zr = nullptr;  // [P][mvpad]  z'_r
   // scratch reused across sweeps
   mutable ffp::Scratch<double> terms;
   mutable ffp::Scratch<double> freqs;
@@ -246,30 +246,6 @@ int build_res_packets(fastfp_pack* pk, int64_t R, const double* d_res, cudaStrea
 void res_release(fastfp_pack* pk);
 // the pulsars of each kernel configuration as Groups with their indices on the device, appended to *out
 int upload_groups(const std::map<KernelCfg, std::vector<int>>& groups, std::vector<Group>* out);
-// fp_sweep*.cu
-struct NmfpOut {      // stage-A outputs of the nmfp path (null for plain Fp)
-  double* Z;          // [P][ceil(F/32)][mvpad/4][8][32]  z'_s, z'_c tiles in MMA B-fragment order
-  double* A;          // [P][ceil(F/32)][5][32]           a_ss, a_sc, a_cc, a_sr, a_cr
-  int mvmax;          // padded width of the per-draw block (multiple of 8)
-};
-int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, double* d_terms,
-                    cudaStream_t st, const NmfpOut* nm = nullptr, double* d_inner = nullptr, bool rest_only = false);
-// the sweep on the path(s) the pack is set to: the tensor kernel for the pulsars it takes, the fp64 kernel for the rest
-int launch_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, double* d_terms, cudaStream_t st,
-                 const NmfpOut* nm = nullptr, double* d_inner = nullptr);
-int launch_reduce_terms(const double* d_terms, int P, int64_t F, double* d_out, cudaStream_t st);
-// residual batches: the sweep over the pack's residual packets (terms [R][P][F]) and the pulsar sum of each row
-// into out[k * ld + f]; with d_minner the sweep writes the Fe inner products instead (fp_sweep.cu)
-int launch_fp_sweep_res(const fastfp_pack* pk, const double* d_freqs, int64_t F, double* d_terms, cudaStream_t st,
-                        double* d_minner = nullptr);
-int launch_reduce_terms_rows(const double* d_terms, int R, int P, int64_t F, double* d_out, int64_t ld,
-                             cudaStream_t st);
-// fp_sweep_i8.cu
-bool i8_eligible(const fastfp_pack* pk);
-int build_i8_planes(fastfp_pack* pk, cudaStream_t st);
-int run_i8_peak(int kind, int iters, double* tops, double* ms);
-int launch_fp_sweep_i8(const fastfp_pack* pk, const double* d_freqs, int64_t F, double* d_terms, cudaStream_t st,
-                       double* d_inner = nullptr, const NmfpOut* nm = nullptr);
 // fe.cu
 int launch_fe_combine(const double* d_inner, int P, int64_t F, const double* d_fplus, const double* d_fcross, int64_t S,
                       double* d_out, int64_t out_ld, cudaStream_t st);
@@ -350,6 +326,34 @@ __device__ __forceinline__ void fence_proxy_async() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
+// ---- warp-specialised kernels: moving registers between warp roles -------------------------
+template <int R>
+__device__ __forceinline__ void reg_alloc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R>
+__device__ __forceinline__ void reg_dealloc() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
+
+// ---- fp64 MMA -------------------------------------------------------------------------------
+// D(8x8) += A(8x4) . B(4x8). Lane l holds A[l>>2][l&3], B[l&3][l>>2], D[l>>2][2*(l&3)+{0,1}].
+__device__ __forceinline__ void dmma_m8n8k4(double& d0, double& d1, double a, double b) {
+  asm("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
+      : "+d"(d0), "+d"(d1)
+      : "d"(a), "d"(b));
+}
+// D(16x8) += A(16x4) . B(4x8). With g = l>>2, t = l&3, lane l holds A[g][t], A[g+8][t] (a0, a1), B[t][g] (b),
+// D[g][2t+{0,1}] (d0, d1) and D[g+8][2t+{0,1}] (d2, d3).
+__device__ __forceinline__ void dmma_m16n8k4(double (&d)[4], double a0, double a1, double b) {
+  asm("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+      : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
+      : "d"(a0), "d"(a1), "d"(b));
+}
+
+// the quiet NaN the statistics return where they are undefined (f <= 0, an empty sky maximum)
+__device__ __forceinline__ double kNaN() { return __longlong_as_double(0x7ff8000000000000LL); }
+
 // One pulsar's term 0.5 N^T M^-1 N with M = [[m00, m01], [m01, m11]], N = [n0, n1], by LU with partial pivoting like
 // jnp.linalg.solve (fastfp.py:90, nmfp.py:117). Where M is singular to the last bit (the Earth-term basis lies inside
 // span(T), e.g. at f = 1/yr against fitted yearly sinusoids) a pivot is exactly zero; the unknown it would divide out is
@@ -367,6 +371,110 @@ __device__ __forceinline__ double term_2x2(double m00, double m01, double m11, d
   const double x1 = u != 0.0 ? (n1 - lq * n0) / u : 0.0;
   const double x0 = m00 != 0.0 ? (n0 - m01 * x1) / m00 : 0.0;
   return 0.5 * (N0 * x0 + N1 * x1);
+}
+
+// ---- the sweep's outputs, one block per mode (DESIGN.md sections 4, 5, 5d, 5e) --------------
+// Both sweep kernels write through these. The caller passes the sizes of the launch -- F frequencies, the row length of
+// every output, and nt32 = ceil(F / 32) -- and the frequency value fq, by reference so that it is read where the
+// writer tests it. At f <= 0 every
+// output of a frequency is NaN, like f**(1/3): Fe is even in f (s flips sign), so without it f < 0 would give Fe(|f|).
+
+// plain Fp / Fe: the term [P][F] and the inner products [P][F][5] (s|s), (s|c), (c|c), (s|r), (c|r); either may be null
+struct FpOut {
+  double* terms;
+  double* inner;
+  // M = [[ss, sc],[sc, cc]], N = [sr, cr]; no f^(-1/3) prefactor: it cancels in every statistic
+  __device__ __forceinline__ void put(int p, int64_t f, int64_t F, const double& fq, double ss, double sc, double cc,
+                                      double sr, double cr) const {
+    double val = term_2x2(ss, sc, cc, sr, cr);
+    if (!(fq > 0.0)) val = kNaN();
+    if (terms) terms[(size_t)p * F + f] = val;
+    if (inner) {
+      double* o = inner + ((size_t)p * F + f) * 5;
+      o[0] = ss; o[1] = sc; o[2] = cc; o[3] = sr; o[4] = cr;
+      if (!(fq > 0.0)) {
+#pragma unroll
+        for (int k = 0; k < 5; ++k) o[k] = kNaN();
+      }
+    }
+  }
+};
+
+// nmfp stage A, per 32-frequency tile: z'_s, z'_c of the per-draw rows,
+// Z [P][nt32][mvpad/4][8][32], and the draw-independent a-terms a_ss, a_sc, a_cc (fixed block removed), a_sr, a_cr,
+// A [P][nt32][5][32]
+struct NmfpTiles {
+  double* Z;
+  double* A;
+  int mvpad;  // per-draw block width padded to the stage-B tile; rows follow the top padding
+  // the z' sin slot of (pulsar p, frequency f, row jr of the padded block); cos is +16. MMA B-fragment order: k-block
+  // (jr / 4), column block (4 frequencies), then 16 * {sin, cos} + 4 * (f % 4) + jr % 4 -- what stage B loads
+  // without bank conflicts
+  __device__ __forceinline__ double* z(int p, int64_t f, int64_t nt32, int jr) const {
+    const int fi = (int)(f & 31);
+    return Z + ((size_t)p * nt32 + (f >> 5)) * ((size_t)mvpad * 64) +
+           (size_t)(((jr >> 2) * 8 + (fi >> 2)) * 32 + 4 * (fi & 3) + (jr & 3));
+  }
+  __device__ __forceinline__ void put_a(int p, int64_t f, int64_t nt32, double ss, double sc, double cc, double sr,
+                                        double cr) const {
+    double* o = A + ((size_t)p * nt32 + (f >> 5)) * 160 + (f & 31);
+    o[0] = ss; o[32] = sc; o[64] = cc; o[96] = sr; o[128] = cr;
+  }
+};
+
+// residual batches of R realisations: Fp terms [R][P][F], or (Fe) x = (s|r_k), (c|r_k) as [F][P][R][2] and
+// mi = (s|s), (s|c), (c|c) as [F][P][3]; the pointers of the other kind are null
+struct ResOut {
+  double* terms;
+  double* x;
+  double* mi;
+  int R, P;
+  __device__ __forceinline__ void put_m(int p, int64_t f, const double& fq, double ss, double sc, double cc) const {
+    if (!mi) return;
+    double* o = mi + ((size_t)f * P + p) * 3;
+    const bool fpos = fq > 0.0;
+    o[0] = fpos ? ss : kNaN();
+    o[1] = fpos ? sc : kNaN();
+    o[2] = fpos ? cc : kNaN();
+  }
+  // realisation k: M = [[m00, m01],[m01, m11]], N = [sr, cr]
+  __device__ __forceinline__ void put(int k, int p, int64_t f, int64_t F, const double& fq, double m00, double m01,
+                                      double m11, double sr, double cr) const {
+    const bool fpos = fq > 0.0;
+    if (x) {
+      *reinterpret_cast<double2*>(x + (((size_t)f * P + p) * R + k) * 2) =
+          fpos ? make_double2(sr, cr) : make_double2(kNaN(), kNaN());
+      return;
+    }
+    double val = term_2x2(m00, m01, m11, sr, cr);
+    if (!fpos) val = kNaN();
+    terms[((size_t)k * P + p) * F + f] = val;
+  }
+};
+
+// ---- sweep launchers (fp_sweep*.cu), each with the output block of its mode ----------------
+int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, const FpOut& out, cudaStream_t st,
+                    bool rest_only = false);
+int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, const NmfpTiles& out, cudaStream_t st,
+                    bool rest_only = false);
+int launch_reduce_terms(const double* d_terms, int P, int64_t F, double* d_out, cudaStream_t st);
+// residual batches: the sweep over the pack's residual packets and the pulsar sum of each row of its [R][P][F] terms
+// into out[k * ld + f] (fp_sweep.cu)
+int launch_fp_sweep_res(const fastfp_pack* pk, const double* d_freqs, int64_t F, const ResOut& out, cudaStream_t st);
+int launch_reduce_terms_rows(const double* d_terms, int R, int P, int64_t F, double* d_out, int64_t ld,
+                             cudaStream_t st);
+// fp_sweep_i8.cu
+bool i8_eligible(const fastfp_pack* pk);
+int build_i8_planes(fastfp_pack* pk, cudaStream_t st);
+int run_i8_peak(int kind, int iters, double* tops, double* ms);
+int launch_fp_sweep_i8(const fastfp_pack* pk, const double* d_freqs, int64_t F, const FpOut& out, cudaStream_t st);
+int launch_fp_sweep_i8(const fastfp_pack* pk, const double* d_freqs, int64_t F, const NmfpTiles& out, cudaStream_t st);
+// the sweep on the path(s) the pack is set to: the tensor kernel for the pulsars it takes, the fp64 kernel for the rest
+template <class Out>  // FpOut or NmfpTiles
+int launch_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, const Out& out, cudaStream_t st) {
+  if (!pk->use_i8()) return launch_fp_sweep(pk, d_freqs, F, out, st);
+  if (int rc = launch_fp_sweep_i8(pk, d_freqs, F, out, st)) return rc;
+  return pk->i8_all() ? 0 : launch_fp_sweep(pk, d_freqs, F, out, st, true);
 }
 
 }  // namespace ffp

@@ -35,73 +35,66 @@ __global__ void reduce_terms_kernel(const double* __restrict__ terms, int P, int
   out[f] = acc;
 }
 
-static int dispatch_group(const fastfp_pack* pk, const Group& g, const SweepArgs& a, bool nmfp, bool res,
-                          cudaStream_t st) {
-  if (g.cfg.wmw == 8) return dispatch_sweep_xwide(pk, g, a, nmfp, res, st);
-  if (g.cfg.wmw == 4) return dispatch_sweep_wide(pk, g, a, nmfp, res, st);
-  if (g.cfg.wmw == 1 && g.cfg.nnb == 4) return dispatch_sweep_w1(pk, g, a, nmfp, res, st);
-  if (g.cfg.wmw == 1) return dispatch_sweep_w2(pk, g, a, nmfp, res, st);
-  return dispatch_sweep_w4(pk, g, a, nmfp, res, st);
+static int dispatch_group(const fastfp_pack* pk, const Group& g, const SweepArgs& a, SweepMode mode, cudaStream_t st) {
+  if (g.cfg.wmw == 8) return dispatch_sweep_xwide(pk, g, a, mode, st);
+  if (g.cfg.wmw == 4) return dispatch_sweep_wide(pk, g, a, mode, st);
+  if (g.cfg.wmw == 1 && g.cfg.nnb == 4) return dispatch_sweep_w1(pk, g, a, mode, st);
+  if (g.cfg.wmw == 1) return dispatch_sweep_w2(pk, g, a, mode, st);
+  return dispatch_sweep_w4(pk, g, a, mode, st);
 }
 
-int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, double* d_terms,
-                    cudaStream_t st, const NmfpOut* nm, double* d_inner, bool rest_only) {
-#ifdef FFP_DEBUG_SWITCHES  // profiling builds only; the shipped library is compiled without it
-  static const int dbg = getenv("FASTFP_DBG") ? atoi(getenv("FASTFP_DBG")) : 0;
-#endif
+static SweepArgs sweep_args(const double* packets, const PulsarMeta* meta, const fastfp_pack* pk,
+                            const double* d_freqs, int64_t F) {
   SweepArgs a{};
-  a.packets = pk->d_packets;
-  a.meta = pk->d_meta;
+  a.packets = packets;
+  a.meta = meta;
   a.freqs = d_freqs;
   a.F = F;
-  a.terms = d_terms;
-  a.inner = d_inner;
   a.slab = pk->d_slab;
   a.counter = pk->d_counter;
-  a.Z = nm ? nm->Z : nullptr;
-  a.A = nm ? nm->A : nullptr;
-  a.mvmax = nm ? nm->mvmax : 0;
-  a.done_mask = pk->d_done_mask;
-#ifdef FFP_DEBUG_SWITCHES
+  return a;
+}
+
+// the pack's sweep in mode Fp or Nmfp; rest_only: only the pulsars the tensor sweep left out
+static int launch_fp_groups(const fastfp_pack* pk, SweepArgs a, SweepMode mode, bool rest_only, cudaStream_t st) {
+#ifdef FFP_DEBUG_SWITCHES  // profiling builds only; the shipped library is compiled without it
+  static const int dbg = getenv("FASTFP_DBG") ? atoi(getenv("FASTFP_DBG")) : 0;
   a.dbg = dbg;
 #endif
+  a.done_mask = pk->d_done_mask;
   for (const Group& g0 : pk->groups) {
     Group g = g0;
-    if (rest_only) {  // only the pulsars the tensor sweep left out
+    if (rest_only) {
       if (g0.count_rest == 0) continue;
       g.count = g0.count_rest;
       g.d_pidx = g0.d_pidx_rest;
     }
-    if (int rc = dispatch_group(pk, g, a, nm != nullptr, false, st)) return rc;
+    if (int rc = dispatch_group(pk, g, a, mode, st)) return rc;
   }
   return 0;
 }
 
-int launch_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, double* d_terms, cudaStream_t st,
-                 const NmfpOut* nm, double* d_inner) {
-  if (!pk->use_i8()) return launch_fp_sweep(pk, d_freqs, F, d_terms, st, nm, d_inner);
-  if (int rc = launch_fp_sweep_i8(pk, d_freqs, F, d_terms, st, d_inner, nm)) return rc;
-  return pk->i8_all() ? 0 : launch_fp_sweep(pk, d_freqs, F, d_terms, st, nm, d_inner, true);
+int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, const FpOut& out, cudaStream_t st,
+                    bool rest_only) {
+  SweepArgs a = sweep_args(pk->d_packets, pk->d_meta, pk, d_freqs, F);
+  a.fp = out;
+  return launch_fp_groups(pk, a, SweepMode::Fp, rest_only, st);
 }
 
-// The residual batch (DESIGN.md section 5d): the fp64 kernel on the pack's residual packets, whose G tiles carry
-// the realisations' w_k as extra rows; terms is [R][P][F]. With d_minner (DESIGN.md section 5e) the kernel writes inner
-// products instead: d_terms gets (s|r_k), (c|r_k) as [F][P][R][2] and d_minner (s|s), (s|c), (c|c) as [F][P][3].
-int launch_fp_sweep_res(const fastfp_pack* pk, const double* d_freqs, int64_t F, double* d_terms, cudaStream_t st,
-                        double* d_minner) {
-  SweepArgs a{};
-  a.packets = pk->d_res_packets;
-  a.meta = pk->d_res_meta;
-  a.freqs = d_freqs;
-  a.F = F;
-  a.terms = d_terms;
-  a.inner = d_minner;
-  a.slab = pk->d_slab;
-  a.counter = pk->d_counter;
-  a.nres = (int)pk->res_R;
-  a.npsr = pk->P;
+int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, const NmfpTiles& out, cudaStream_t st,
+                    bool rest_only) {
+  SweepArgs a = sweep_args(pk->d_packets, pk->d_meta, pk, d_freqs, F);
+  a.nm = out;
+  return launch_fp_groups(pk, a, SweepMode::Nmfp, rest_only, st);
+}
+
+// The residual batch (DESIGN.md sections 5d, 5e): the fp64 kernel on the pack's residual packets, whose G tiles carry
+// the realisations' w_k as extra rows
+int launch_fp_sweep_res(const fastfp_pack* pk, const double* d_freqs, int64_t F, const ResOut& out, cudaStream_t st) {
+  SweepArgs a = sweep_args(pk->d_res_packets, pk->d_res_meta, pk, d_freqs, F);
+  a.res = out;
   for (const Group& g : pk->res_groups)
-    if (int rc = dispatch_group(pk, g, a, false, true, st)) return rc;
+    if (int rc = dispatch_group(pk, g, a, SweepMode::Res, st)) return rc;
   return 0;
 }
 

@@ -69,11 +69,8 @@ struct Args {
   const int* pidx;
   const double* freqs;
   int64_t F;
-  double* terms;                 // [P][F]
-  double* inner;                 // optional [P][F][5]: (s|s), (s|c), (c|c), (s|r), (c|r); null = terms only
-  double* Z;                     // nmfp stage A: [P][ceil(F/32)][mvpad/4][8][32] z'_s, z'_c tiles (B-fragment order)
-  double* A;                     // nmfp stage A: [P][ceil(F/32)][5][32] a_ss, a_sc, a_cc, a_sr, a_cr
-  int mvpad;
+  FpOut fp;                      // fp_sweep_i8_kernel<false>
+  NmfpTiles nm;                  // fp_sweep_i8_kernel<true>: nmfp stage A
   int ntile, nwork;              // 16-frequency tiles per pulsar, work items
   int nt32;                      // 32-frequency tiles of the nmfp outputs
   int gslot, gst;                // G ring: bytes per slot (7 x rows_max x 32), number of slots
@@ -196,10 +193,6 @@ __device__ __forceinline__ void wgmma_i8(uint32_t (&d)[NACC], uint64_t da, uint6
         "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
       : "l"(da), "l"(db), "r"(accumulate));
 }
-template <int R>
-__device__ __forceinline__ void reg_set_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
-template <int R>
-__device__ __forceinline__ void reg_set_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // x in [-1, 1] -> the 7 bytes of Q + 0x80..80, Q = rint(x 2^54), every byte XORed with 0x80: balanced signed digits,
 // most significant in byte 6. The scaling is an integer add on the exponent field (zero and subnormals land below
@@ -310,7 +303,7 @@ __global__ void __launch_bounds__(THREADS, 1) fp_sweep_i8_kernel(const Args ar) 
 
   if (wid < 4) {
     // ================= control warpgroup: TMA (warp 0, lane 0) =================
-    reg_set_dec<REGS_CTRL>();
+    reg_dealloc<REGS_CTRL>();
     if (wid == 0 && lane == 0) {
       // ring positions and phase parities are carried incrementally (no division by the runtime ring depth per stage)
       uint32_t k = 0, sv = 0, vpar = 0, sg = 0, gpar = 0;
@@ -340,7 +333,7 @@ __global__ void __launch_bounds__(THREADS, 1) fp_sweep_i8_kernel(const Args ar) 
     }
   } else if (wid < 12) {
     // ================= consumer warpgroups: wgmma issue + epilogue, 64 operand rows each =================
-    reg_set_inc<REGS_CONS>();
+    reg_alloc<REGS_CONS>();
     const int cwg = (wid - 4) >> 2;          // operand rows 64 cwg .. 64 cwg + 63 of the row group
     const int cw = (wid - 4) & 3;            // warp inside the warpgroup: 16 of those rows
     const int lr0 = 64 * cwg + 16 * cw + (lane >> 2);  // accumulator rows lr0 and lr0 + 8 of this thread
@@ -405,11 +398,8 @@ __global__ void __launch_bounds__(THREADS, 1) fp_sweep_i8_kernel(const Args ar) 
                 sm.nval[2 * fl + 1] = yc;
               }
               if (NMFP && row >= pm.mfix && row < pm.m && f0 + fl < ar.F) {
-                // rows of the per-draw block leave as z' in the layout nmfp_stageB_kernel streams: 32-frequency tile,
-                // k-block (row / 4), column block (4 frequencies), then 16 * {sin, cos} + 4 * (frequency % 4) + row % 4
-                const int jr = row - pm.mfix + (ar.mvpad - pm.mvar), fi = (int)((f0 + fl) & 31);
-                double* z = ar.Z + ((size_t)p * ar.nt32 + (size_t)((f0 + fl) >> 5)) * ((size_t)ar.mvpad * 64) +
-                            (size_t)(((jr >> 2) * 8 + (fi >> 2)) * 32 + 4 * (fi & 3) + (jr & 3));
+                // rows of the per-draw block leave as z'
+                double* z = ar.nm.z(p, f0 + fl, ar.nt32, row - pm.mfix + (ar.nm.mvpad - pm.mvar));
                 z[0] = ys;
                 z[16] = yc;
               }
@@ -458,25 +448,10 @@ __global__ void __launch_bounds__(THREADS, 1) fp_sweep_i8_kernel(const Args ar) 
           for (int k2 = 0; k2 < 2; ++k2)
             a[k2] = sm.redA[((buf * 2 + 0) * NF + f) * 3 + k2] + sm.redA[((buf * 2 + 1) * NF + f) * 3 + k2];
           a[2] = pm.ninv_sum - a[0];  // c N^-1 c = sum 1/N - s N^-1 s (s^2 + c^2 = 1 to the last bit of the sincos values)
-          const double N0 = sm.nval[2 * f], N1 = sm.nval[2 * f + 1];
-          // M = [[ss, sc],[sc, cc]], N = [(s|r), (c|r)]
-          double val = term_2x2(a[0] - b[0], a[1] - b[1], a[2] - b[2], N0, N1);
-          if (NMFP) {
-            if (fidx < ar.F) {  // the draw-independent pieces (fixed block removed) for stage B
-              double* o = ar.A + ((size_t)p * ar.nt32 + (size_t)(fidx >> 5)) * 160 + (fidx & 31);
-              o[0] = a[0] - b[0]; o[32] = a[1] - b[1]; o[64] = a[2] - b[2]; o[96] = N0; o[128] = N1;
-            }
-          } else if (fidx < ar.F) {
-            if (!(ar.freqs[fidx] > 0.0)) val = __longlong_as_double(0x7ff8000000000000LL);  // f <= 0: NaN like f**(1/3)
-            if (ar.terms) ar.terms[(size_t)p * ar.F + fidx] = val;
-            if (ar.inner) {
-              double* o = ar.inner + ((size_t)p * ar.F + fidx) * 5;
-              o[0] = a[0] - b[0]; o[1] = a[1] - b[1]; o[2] = a[2] - b[2]; o[3] = N0; o[4] = N1;
-              if (!(ar.freqs[fidx] > 0.0)) {  // f <= 0: NaN like f**(1/3) (Fe is even in f)
-#pragma unroll
-                for (int k = 0; k < 5; ++k) o[k] = __longlong_as_double(0x7ff8000000000000LL);
-              }
-            }
+          const double N0 = sm.nval[2 * f], N1 = sm.nval[2 * f + 1];  // (s|r), (c|r)
+          if (fidx < ar.F) {
+            if (NMFP) ar.nm.put_a(p, fidx, ar.nt32, a[0] - b[0], a[1] - b[1], a[2] - b[2], N0, N1);
+            else ar.fp.put(p, fidx, ar.F, ar.freqs[fidx], a[0] - b[0], a[1] - b[1], a[2] - b[2], N0, N1);
           }
         }
         __syncwarp();
@@ -486,7 +461,7 @@ __global__ void __launch_bounds__(THREADS, 1) fp_sweep_i8_kernel(const Args ar) 
     }
   } else {
     // ================= producers: sin/cos digit planes + the two quadratic sums =================
-    reg_set_dec<REGS_PROD>();
+    reg_dealloc<REGS_PROD>();
     const int pw = wid - 12;
     const uint32_t grp = (uint32_t)(pw >> 2);          // serves the stages with (global stage index % 2) == grp
     // lane = 4 * kg + fl: the 8 lanes of a quarter-warp read two distinct (t, 1/N) entries 64 bytes apart (no bank
@@ -812,26 +787,24 @@ int build_i8_planes(fastfp_pack* pk, cudaStream_t st) {
   return 0;
 }
 
-int launch_fp_sweep_i8(const fastfp_pack* pk, const double* d_freqs, int64_t F, double* d_terms, cudaStream_t st,
-                       double* d_inner, const NmfpOut* nm) {
+// one of fp, nm is set
+static int launch_i8(const fastfp_pack* pk, const double* d_freqs, int64_t F, const FpOut* fp, const NmfpTiles* nm,
+                     cudaStream_t st) {
   using namespace i8;
   Args a{};
+  a.freqs = d_freqs;
+  a.F = F;
+  if (fp) a.fp = *fp;
+  if (nm) a.nm = *nm;
   a.planes = pk->d_i8;
   a.rowscale = pk->d_i8_scale;
   a.meta = pk->d_meta;
   a.pidx = pk->d_pidx_all;
-  a.freqs = d_freqs;
-  a.F = F;
-  a.terms = d_terms;
-  a.inner = d_inner;
-  a.Z = nm ? nm->Z : nullptr;
-  a.A = nm ? nm->A : nullptr;
-  a.mvpad = nm ? nm->mvmax : 0;
-  const int64_t ntile = (F + NF - 1) / NF, nwork = ntile * pk->i8_count;  // the pulsars this kernel takes
+  const int64_t ntile = (a.F + NF - 1) / NF, nwork = ntile * pk->i8_count;  // the pulsars this kernel takes
   if (nwork > 0x7fffffffLL) { set_error("frequency batch too large for one launch"); return -1; }
   a.ntile = (int)ntile;
   a.nwork = (int)nwork;
-  a.nt32 = (int)((F + 31) / 32);
+  a.nt32 = (int)((a.F + 31) / 32);
   a.gslot = NPL * (pk->i8_rows_max < 128 ? pk->i8_rows_max : 128) * KT;  // one row group
   const size_t budget = 220 * 1024 - SMEM_FIXED;
   int gst = (int)(budget / a.gslot);
@@ -852,6 +825,14 @@ int launch_fp_sweep_i8(const fastfp_pack* pk, const double* d_freqs, int64_t F, 
   g_launches += 1;
   FFP_CUDA(cudaGetLastError());
   return 0;
+}
+
+int launch_fp_sweep_i8(const fastfp_pack* pk, const double* d_freqs, int64_t F, const FpOut& out, cudaStream_t st) {
+  return launch_i8(pk, d_freqs, F, &out, nullptr, st);
+}
+int launch_fp_sweep_i8(const fastfp_pack* pk, const double* d_freqs, int64_t F, const NmfpTiles& out,
+                       cudaStream_t st) {
+  return launch_i8(pk, d_freqs, F, nullptr, &out, st);
 }
 
 }  // namespace ffp

@@ -3,7 +3,7 @@
 // per SM -- takes (pulsar, frequency-tile) work items from an atomic counter.
 //
 // Replaces the body of FastFp.calculate_Fp under jax.vmap (reference fastfp/fastfp.py:69-92,
-// examples/run_fp.py:63) -- and, with NMFP = true, the draw-independent part of
+// examples/run_fp.py:63) -- and, in SweepMode::Nmfp, the draw-independent part of
 // NMFP.calculate_nmfp (fastfp/nmfp.py:96-119) -- for a whole frequency tile at once:
 //
 //   per chunk of CI TOAs
@@ -38,6 +38,8 @@
 
 namespace ffp {
 
+enum class SweepMode { Fp, Nmfp, Res };  // which output block the kernel writes
+
 struct SweepArgs {
   const double* packets;
   const PulsarMeta* meta;
@@ -46,18 +48,17 @@ struct SweepArgs {
   int nwork;
   const double* freqs;
   int64_t F;
-  double* terms;          // [P][F] (plain Fp)
-  double* inner;          // optional [P][F][5]: (s|s), (s|c), (c|c), (s|r), (c|r) (Fe-statistic); null = terms only
+  // the output block of the kernel's mode (the realisations of SweepMode::Res are rows roundup8(m) .. roundup8(m)+R-1
+  // of G). A union, since a kernel writes one: a parameter block of more than 128 bytes is read through a pointer
+  // instead of straight from the constant bank, which changes the code of the whole kernel.
+  union {
+    FpOut fp;
+    NmfpTiles nm;
+    ResOut res;
+  };
   double* slab;           // level-2 scratch, SLAB doubles per CTA
   unsigned int* counter;  // work counter (zeroed before the launch)
-  double* Z;              // nmfp: [P][ceil(F/32)][mvmax/4][8][32] (B-fragment order, mvmax = padded)
-  double* A;              // nmfp: [P][ceil(F/32)][5][32]
-  int mvmax;
   const unsigned char* done_mask;  // block-N packs: per chunk, which of the 8 epoch slots end there
-  // residual batches: realisations, in rows roundup8(m) .. roundup8(m)+nres-1 of G; terms is [nres][npsr][F], or with
-  // inner set (Fe over residual batches) terms is [F][npsr][nres][2] ((s|r_k), (c|r_k)) and inner is [F][npsr][3]
-  int nres;
-  int npsr;
 #ifdef FFP_DEBUG_SWITCHES
   int dbg;  // profiling builds only (tools/dbg_split.sh): bit 0 producers' math off, 1 MMAs off, 2 level-2 flush off
 #endif
@@ -69,21 +70,6 @@ struct SweepArgs {
 #define FFP_DBG(ar, bit) 0
 #endif
 
-// D(16x8) += A(16x4) . B(4x8), fp64. With g = l>>2, t = l&3, lane l holds A[g][t], A[g+8][t] (a0, a1), B[t][g] (b),
-// D[g][2t+{0,1}] (d0, d1) and D[g+8][2t+{0,1}] (d2, d3).
-__device__ __forceinline__ void dmma_m16n8k4(double (&d)[4], double a0, double a1, double b) {
-  asm("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
-      : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
-      : "d"(a0), "d"(a1), "d"(b));
-}
-template <int R>
-__device__ __forceinline__ void reg_alloc() {
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
-}
-template <int R>
-__device__ __forceinline__ void reg_dealloc() {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
-}
 // Shared-memory carve-up, identical for both roles.
 template <class C>
 struct SweepSmem {
@@ -114,7 +100,7 @@ struct WorkItem {
 };
 
 // ---- producer role: sin/cos tiles + the five weighted sums -----------------------------------
-template <class C, bool NMFP, bool ECORR>
+template <class C>
 __device__ __forceinline__ void producer_loop(const SweepArgs& ar, SweepSmem<C>& sm, volatile int* s_work,
                                               const int pw, const int lane) {
   constexpr int CI = C::CI, XW = C::XW;
@@ -264,10 +250,35 @@ __device__ __forceinline__ void producer_loop(const SweepArgs& ar, SweepSmem<C>&
   }
 }
 
+// Residual batches (DESIGN.md section 5d): rows from roundup8(m) on hold w_k = C^-1 r_k, so Y there is ((s|r_k),
+// (c|r_k)); one 2x2 system per (realisation, frequency) with the M of the frequency, which redB[fl][3] holds.
+// acc[r][q]: as in consumer_loop's epilogue.
+template <class C>
+__device__ __forceinline__ void res_tail(const ResOut& out, int64_t F, const SweepSmem<C>& sm,
+                                         const double (&acc)[C::NMBW][C::NNB / 2][4], const double* redB, int p,
+                                         int64_t f0, int m, int wm, int wn, int lane) {
+  constexpr int NMBW = C::NMBW, NMT = C::NNB / 2;
+  asm volatile("bar.sync 1, %0;" ::"n"(C::NTC) : "memory");  // consumers only: M of every frequency is published
+  const int r0 = (m + 7) & ~7;
+#pragma unroll
+  for (int q = 0; q < NMT; ++q) {
+    const int fl = 8 * (wn * NMT + q) + (lane >> 2);
+    const int64_t f = f0 + fl;
+    if (f >= F) continue;
+    const double m00 = redB[fl * 3], m01 = redB[fl * 3 + 1], m11 = redB[fl * 3 + 2], fq = sm.fq[fl];
+#pragma unroll
+    for (int r = 0; r < NMBW; ++r)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int k = 8 * (wm * NMBW + r) + 2 * (lane & 3) + e - r0;
+      if (k < 0 || k >= out.R) continue;
+      out.put(k, p, f, F, fq, m00, m01, m11, acc[r][q][e], acc[r][q][2 + e]);
+    }
+  }
+}
+
 // ---- consumer role: the contraction and the epilogue -----------------------------------------
-// RES: residual batches (DESIGN.md section 5d). Rows from roundup8(m) on hold w_k = C^-1 r_k, so Y there is
-// ((s|r_k), (c|r_k)); the epilogue solves one 2x2 system per (realisation, frequency) with the shared M.
-template <class C, bool NMFP, bool ECORR, bool RES>
+template <class C, SweepMode MODE, bool ECORR>
 __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>& sm, volatile int* s_work,
                                               const int cw, const int lane) {
   // a warp owns NMBW blocks of 8 basis rows (the N side, B = G^T) x NMT tiles of 8 frequencies x {sin, cos} (the M
@@ -471,16 +482,11 @@ __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>&
           ps[e][0] = fma(ys, ys, ps[e][0]);
           ps[e][1] = fma(ys, yc, ps[e][1]);
           ps[e][2] = fma(yc, yc, ps[e][2]);
-        } else if (NMFP && j < pm.m) {
-          // nmfp: rows of the per-draw block go out as z' (canonical 32-frequency tiles)
+        } else if (MODE == SweepMode::Nmfp && j < pm.m) {
+          // nmfp: rows of the per-draw block go out as z'
           const int64_t f = f0 + 8 * (wn * NMT + q) + (lane >> 2);
           if (f < ar.F) {
-            // 32-frequency tile, MMA B-fragment order: k-block (row/4), column block (4 freqs), then
-            // position 16*sc + 4*(freq%4) + row%4 -- the layout stage B loads without conflicts
-            const int64_t nt32 = (ar.F + 31) >> 5;
-            const int jr = j - mfix + (ar.mvmax - pm.mvar), fi = (int)(f & 31);  // rows follow the top padding
-            double* z = ar.Z + ((size_t)p * nt32 + (f >> 5)) * ((size_t)ar.mvmax * 64) +
-                        (size_t)(((jr >> 2) * 8 + (fi >> 2)) * 32 + 4 * (fi & 3) + (jr & 3));
+            double* z = ar.nm.z(p, f, (ar.F + 31) >> 5, j - mfix + (ar.nm.mvpad - pm.mvar));
             z[0] = ys;
             z[16] = yc;
           }
@@ -509,76 +515,24 @@ __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>&
       for (int g2 = 0; g2 < C::KSPLIT; ++g2)
 #pragma unroll
         for (int k = 0; k < 5; ++k) a[k] += redA[(g2 * C::KF + tid) * 5 + k];
-      if (NMFP) {
-        // draw-independent pieces: a_ss, a_sc, a_cc (fixed block removed), a_sr, a_cr
-        const int64_t nt32 = (ar.F + 31) >> 5;
-        double* o = ar.A + ((size_t)p * nt32 + (fidx >> 5)) * 160 + (fidx & 31);
-        o[0] = a[0] - b[0];
-        o[32] = a[1] - b[1];
-        o[64] = a[2] - b[2];
-        o[96] = a[3];
-        o[128] = a[4];
-      } else if (RES) {
+      if (MODE == SweepMode::Fp) ar.fp.put(p, fidx, ar.F, sm.fq[tid], a[0] - b[0], a[1] - b[1], a[2] - b[2], a[3], a[4]);
+      if (MODE == SweepMode::Nmfp) ar.nm.put_a(p, fidx, (ar.F + 31) >> 5, a[0] - b[0], a[1] - b[1], a[2] - b[2], a[3], a[4]);
+      if (MODE == SweepMode::Res) {
         // M of this frequency for every realisation; slot 0 of redB for this frequency is read by this thread only
         redB[tid * 3 + 0] = a[0] - b[0];
         redB[tid * 3 + 1] = a[1] - b[1];
         redB[tid * 3 + 2] = a[2] - b[2];
-        if (ar.inner) {  // inner-product output: (s|s), (s|c), (c|c) as [F][P][3], NaN at f <= 0 (Fe is even in f)
-          double* o = ar.inner + ((size_t)fidx * ar.npsr + p) * 3;
-          const bool fpos = sm.fq[tid] > 0.0;
-#pragma unroll
-          for (int k = 0; k < 3; ++k) o[k] = fpos ? a[k] - b[k] : __longlong_as_double(0x7ff8000000000000LL);
-        }
-      } else {
-        // M = [[ss, sc],[sc, cc]], N = [(s|r), (c|r)]
-        double val = term_2x2(a[0] - b[0], a[1] - b[1], a[2] - b[2], a[3], a[4]);
-        if (!(sm.fq[tid] > 0.0)) val = __longlong_as_double(0x7ff8000000000000LL);
-        if (ar.terms) ar.terms[(size_t)p * ar.F + fidx] = val;
-        if (ar.inner) {  // the inner products themselves (no f^(-1/3) prefactor: it cancels in every statistic)
-          double* o = ar.inner + ((size_t)p * ar.F + fidx) * 5;
-          o[0] = a[0] - b[0]; o[1] = a[1] - b[1]; o[2] = a[2] - b[2]; o[3] = a[3]; o[4] = a[4];
-          // f <= 0: NaN like f**(1/3). Fe is even in f (s flips sign), so without this f < 0 would give Fe(|f|)
-          if (!(sm.fq[tid] > 0.0)) {
-#pragma unroll
-            for (int k = 0; k < 5; ++k) o[k] = __longlong_as_double(0x7ff8000000000000LL);
-          }
-        }
+        ar.res.put_m(p, fidx, sm.fq[tid], a[0] - b[0], a[1] - b[1], a[2] - b[2]);
       }
     }
-    if (RES) {
-      asm volatile("bar.sync 1, %0;" ::"n"(C::NTC) : "memory");  // consumers only: M of every frequency is published
-      const int r0 = (pm.m + 7) & ~7;
-#pragma unroll
-      for (int q = 0; q < NMT; ++q) {
-        const int fl = 8 * (wn * NMT + q) + (lane >> 2);
-        const int64_t f = f0 + fl;
-        if (f >= ar.F) continue;
-        const double m00 = redB[fl * 3], m01 = redB[fl * 3 + 1], m11 = redB[fl * 3 + 2];
-        const bool fpos = sm.fq[fl] > 0.0;
-#pragma unroll
-        for (int r = 0; r < NMBW; ++r)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int k = 8 * (wm * NMBW + r) + 2 * (lane & 3) + e - r0;
-          if (k < 0 || k >= ar.nres) continue;
-          if (ar.inner) {  // inner-product output: (s|r_k), (c|r_k) as [F][P][R][2]
-            const double nan = __longlong_as_double(0x7ff8000000000000LL);
-            *reinterpret_cast<double2*>(ar.terms + (((size_t)f * ar.npsr + p) * ar.nres + k) * 2) =
-                fpos ? make_double2(acc[r][q][e], acc[r][q][2 + e]) : make_double2(nan, nan);
-            continue;
-          }
-          double val = term_2x2(m00, m01, m11, acc[r][q][e], acc[r][q][2 + e]);
-          if (!fpos) val = __longlong_as_double(0x7ff8000000000000LL);
-          ar.terms[((size_t)k * ar.npsr + p) * ar.F + f] = val;
-        }
-      }
-    }
+    if (MODE == SweepMode::Res) res_tail<C>(ar.res, ar.F, sm, acc, redB, p, f0, pm.m, wm, wn, lane);
     __syncthreads();  // B4: fq, red and s_work are reused by the next work item
   }
 }
 
-template <class C, bool NMFP, bool ECORR, bool RES>
+template <class C, SweepMode MODE, bool ECORR>
 __global__ void __launch_bounds__(C::NTHREADS, CTAS_PER_SM) fp_sweep_kernel(const SweepArgs ar) {
+  static_assert(!(MODE == SweepMode::Res && ECORR), "residual batches are diagonal-N only");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   SweepSmem<C> sm(smem_raw);
   __shared__ int s_work;
@@ -592,19 +546,19 @@ __global__ void __launch_bounds__(C::NTHREADS, CTAS_PER_SM) fp_sweep_kernel(cons
   __syncthreads();
   if (wid < C::NWC) {
     reg_alloc<C::CREGS>();
-    consumer_loop<C, NMFP, ECORR, RES>(ar, sm, &s_work, wid, lane);
+    consumer_loop<C, MODE, ECORR>(ar, sm, &s_work, wid, lane);
   } else {
     reg_dealloc<C::PREGS>();
-    producer_loop<C, NMFP, ECORR>(ar, sm, &s_work, wid - C::NWC, lane);
+    producer_loop<C>(ar, sm, &s_work, wid - C::NWC, lane);
   }
 }
 
 // ---- launch helpers -------------------------------------------------------------------------
-template <class C, bool NMFP, bool ECORR, bool RES>
+template <class C, SweepMode MODE, bool ECORR>
 int launch_sweep_cfg(const fastfp_pack* pk, const Group& g, const SweepArgs& base, cudaStream_t st) {
   static bool attr_done[64] = {};
   if (!attr_done[pk->device & 63]) {
-    FFP_CUDA(cudaFuncSetAttribute(fp_sweep_kernel<C, NMFP, ECORR, RES>,
+    FFP_CUDA(cudaFuncSetAttribute(fp_sweep_kernel<C, MODE, ECORR>,
                                   cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
     attr_done[pk->device & 63] = true;
   }
@@ -618,30 +572,32 @@ int launch_sweep_cfg(const fastfp_pack* pk, const Group& g, const SweepArgs& bas
   const int64_t resident = (int64_t)CTAS_PER_SM * pk->num_sms;
   const unsigned grid = (unsigned)(nwork < resident ? nwork : resident);
   FFP_CUDA(cudaMemsetAsync(a.counter, 0, sizeof(unsigned int), st));
-  fp_sweep_kernel<C, NMFP, ECORR, RES><<<grid, C::NTHREADS, C::SMEM, st>>>(a);
+  fp_sweep_kernel<C, MODE, ECORR><<<grid, C::NTHREADS, C::SMEM, st>>>(a);
   g_launches += 1;
   FFP_CUDA(cudaGetLastError());
   return 0;
 }
 
-// one translation unit per configuration family instantiates these (compile time); res: the residual-batch mode
-// (diagonal-N, plain-Fp packs only)
-int dispatch_sweep_w1(const fastfp_pack*, const Group&, const SweepArgs&, bool nmfp, bool res, cudaStream_t);
-int dispatch_sweep_w2(const fastfp_pack*, const Group&, const SweepArgs&, bool nmfp, bool res, cudaStream_t);
-int dispatch_sweep_w4(const fastfp_pack*, const Group&, const SweepArgs&, bool nmfp, bool res, cudaStream_t);
-int dispatch_sweep_wide(const fastfp_pack*, const Group&, const SweepArgs&, bool nmfp, bool res, cudaStream_t);
-int dispatch_sweep_xwide(const fastfp_pack*, const Group&, const SweepArgs&, bool nmfp, bool res, cudaStream_t);
+// one translation unit per configuration family instantiates these (compile time)
+int dispatch_sweep_w1(const fastfp_pack*, const Group&, const SweepArgs&, SweepMode, cudaStream_t);
+int dispatch_sweep_w2(const fastfp_pack*, const Group&, const SweepArgs&, SweepMode, cudaStream_t);
+int dispatch_sweep_w4(const fastfp_pack*, const Group&, const SweepArgs&, SweepMode, cudaStream_t);
+int dispatch_sweep_wide(const fastfp_pack*, const Group&, const SweepArgs&, SweepMode, cudaStream_t);
+int dispatch_sweep_xwide(const fastfp_pack*, const Group&, const SweepArgs&, SweepMode, cudaStream_t);
 
+// five kernels per configuration: Fp and Nmfp, each with diagonal or block-diagonal N (pk->ecorr), and Res (diagonal N,
+// plain-Fp packs only)
 #define FFP_SWEEP_CASE(NMBWv, NNBv, WMWv, CIv) FFP_SWEEP_CASE_W(NMBWv, NNBv, WMWv, CIv, 8, 16)
 #define FFP_SWEEP_CASE_W(NMBWv, NNBv, WMWv, CIv, NWCv, NWPv)                                       \
   if (g.cfg.nmbw == NMBWv && g.cfg.nnb == NNBv && g.cfg.wmw == WMWv && g.cfg.ci == CIv &&          \
       g.cfg.nwc == NWCv) {                                                                         \
     using Cfg_ = SweepCfg<NMBWv, NNBv, WMWv, CIv, NWCv, NWPv>;                                      \
-    if (res) return launch_sweep_cfg<Cfg_, false, false, true>(pk, g, a, st);                      \
-    if (pk->ecorr) return nmfp ? launch_sweep_cfg<Cfg_, true, true, false>(pk, g, a, st)            \
-                               : launch_sweep_cfg<Cfg_, false, true, false>(pk, g, a, st);          \
-    return nmfp ? launch_sweep_cfg<Cfg_, true, false, false>(pk, g, a, st)                          \
-                : launch_sweep_cfg<Cfg_, false, false, false>(pk, g, a, st);                        \
+    if (mode == SweepMode::Res) return launch_sweep_cfg<Cfg_, SweepMode::Res, false>(pk, g, a, st);  \
+    if (mode == SweepMode::Nmfp)                                                                   \
+      return pk->ecorr ? launch_sweep_cfg<Cfg_, SweepMode::Nmfp, true>(pk, g, a, st)               \
+                       : launch_sweep_cfg<Cfg_, SweepMode::Nmfp, false>(pk, g, a, st);             \
+    return pk->ecorr ? launch_sweep_cfg<Cfg_, SweepMode::Fp, true>(pk, g, a, st)                   \
+                     : launch_sweep_cfg<Cfg_, SweepMode::Fp, false>(pk, g, a, st);                 \
   }
 
 }  // namespace ffp

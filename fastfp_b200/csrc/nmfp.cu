@@ -230,12 +230,6 @@ struct FactorCfg {
   static constexpr size_t SMEM = (size_t)FW * WSZ * 8;
 };
 
-__device__ __forceinline__ void dmma884(double& d0, double& d1, double a, double b) {
-  asm("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-      : "+d"(d0), "+d"(d1)
-      : "d"(a), "d"(b));
-}
-
 // 8x8 Cholesky of the (symmetric) block held in C layout and the inverse of its factor, fused: after
 // step j column j of L is final, which is all that row j of X = L^-1 needs. Returns X in C layout with
 // exact zeros above the diagonal.
@@ -321,7 +315,7 @@ __global__ void __launch_bounds__(FactorCfg<NMBV>::FW * 32, FactorCfg<NMBV>::CTA
     double c0, c1, t0 = 0.0, t1 = 0.0;
     ld_c(blk(j, j), c0, c1);
 #pragma unroll
-    for (int k = 0; k < j; ++k) { dmma884(t0, t1, bj[k][0], bj[k][0]); dmma884(t0, t1, bj[k][1], bj[k][1]); }
+    for (int k = 0; k < j; ++k) { dmma_m8n8k4(t0, t1, bj[k][0], bj[k][0]); dmma_m8n8k4(t0, t1, bj[k][1], bj[k][1]); }
     double x0, x1;
     chol_inv_8x8(c0 - t0, c1 - t1, x0, x1, lane);
     st_c(blk(j, j), x0, x1);
@@ -331,8 +325,8 @@ __global__ void __launch_bounds__(FactorCfg<NMBV>::FW * 32, FactorCfg<NMBV>::CTA
       double u0 = 0.0, u1 = 0.0, v0, v1;
 #pragma unroll
       for (int k = 0; k < j; ++k) {
-        dmma884(u0, u1, blk(i, k)[offA0], bj[k][0]);
-        dmma884(u0, u1, blk(i, k)[offA1], bj[k][1]);
+        dmma_m8n8k4(u0, u1, blk(i, k)[offA0], bj[k][0]);
+        dmma_m8n8k4(u0, u1, blk(i, k)[offA1], bj[k][1]);
       }
       ld_c(blk(i, j), v0, v1);
       st_c(blk(i, j), v0 - u0, v1 - u1);
@@ -348,8 +342,8 @@ __global__ void __launch_bounds__(FactorCfg<NMBV>::FW * 32, FactorCfg<NMBV>::CTA
 #pragma unroll
       for (int i = j + 1; i < NMBV; ++i) {
         double r0 = 0.0, r1 = 0.0;
-        dmma884(r0, r1, pa[i - j - 1][0], bi0);
-        dmma884(r0, r1, pa[i - j - 1][1], bi1);
+        dmma_m8n8k4(r0, r1, pa[i - j - 1][0], bi0);
+        dmma_m8n8k4(r0, r1, pa[i - j - 1][1], bi1);
         st_c(blk(i, j), r0, r1);
       }
       __syncwarp();
@@ -369,8 +363,8 @@ __global__ void __launch_bounds__(FactorCfg<NMBV>::FW * 32, FactorCfg<NMBV>::CTA
       double t0 = 0.0, t1 = 0.0;
 #pragma unroll
       for (int k = j; k < i; ++k) {
-        dmma884(t0, t1, la[k][0], blk(k, j)[offT0]);
-        dmma884(t0, t1, la[k][1], blk(k, j)[offT1]);
+        dmma_m8n8k4(t0, t1, la[k][0], blk(k, j)[offT0]);
+        dmma_m8n8k4(t0, t1, la[k][1], blk(k, j)[offT1]);
       }
       st_c(blk(i, j), t0, t1);
     }
@@ -382,8 +376,8 @@ __global__ void __launch_bounds__(FactorCfg<NMBV>::FW * 32, FactorCfg<NMBV>::CTA
 #pragma unroll
     for (int j = 0; j < i; ++j) {
       double r0 = 0.0, r1 = 0.0;
-      dmma884(r0, r1, nx0, tb[j][0]);
-      dmma884(r0, r1, nx1, tb[j][1]);
+      dmma_m8n8k4(r0, r1, nx0, tb[j][0]);
+      dmma_m8n8k4(r0, r1, nx1, tb[j][1]);
       st_c(blk(i, j), r0, r1);
     }
     __syncwarp();
@@ -402,7 +396,7 @@ __global__ void __launch_bounds__(FactorCfg<NMBV>::FW * 32, FactorCfg<NMBV>::CTA
     for (int mb = kb / 2; mb < NMBV; ++mb, ++b) {
       const double val = blk(mb, kb / 2)[(kb & 1) ? offA1 : offA0];
       out[b * 32 + lane] = val;
-      dmma884(acc[mb][0], acc[mb][1], val, zb);
+      dmma_m8n8k4(acc[mb][0], acc[mb][1], val, zb);
     }
   }
   if (q == 0) {
@@ -491,6 +485,8 @@ __global__ void __launch_bounds__(StageBCfg<NMBV>::THREADS, 1) nmfp_stageB_kerne
 
   // ---- consumers ----
   const int h = w >> 3, wl = w & 7;                  // half-tile, warp inside it
+  // B fragment of lane (k = lane & 3, n = lane >> 2) in one (k-block, column block) of a z' tile, the layout
+  // NmfpTiles::z writes: row k, sin (n even) or cos (n odd) of frequency n / 2 of the column block
   const int bperm = 16 * ((lane >> 2) & 1) + 4 * (lane >> 3) + (lane & 3);
   constexpr int nblk = NMBV * (NMBV + 1);
   const int fi = 4 * wl + (lane & 3);                // this lane group's frequency inside the half-tile
@@ -522,7 +518,7 @@ __global__ void __launch_bounds__(StageBCfg<NMBV>::THREADS, 1) nmfp_stageB_kerne
         const int off = linv_block_off(NMBV, kb);
 #pragma unroll
         for (int mb = kb / 2; mb < NMBV; ++mb)
-          dmma884(acc[mb][0], acc[mb][1], lt[(off + mb - kb / 2) * 32 + lane], b);
+          dmma_m8n8k4(acc[mb][0], acc[mb][1], lt[(off + mb - kb / 2) * 32 + lane], b);
       }
     }
     // u = L^-1 z' for row 8*mb + (lane>>2), frequency fi: [0] = sin, [1] = cos
@@ -557,7 +553,7 @@ __global__ void __launch_bounds__(StageBCfg<NMBV>::THREADS, 1) nmfp_stageB_kerne
   }
   if ((lane >> 2) < nd && f < ar.F) {
     double val = fpacc;
-    if (!(fval > 0.0)) val = __longlong_as_double(0x7ff8000000000000LL);
+    if (!(fval > 0.0)) val = kNaN();
     ar.out[(size_t)(d0 + (lane >> 2)) * ar.out_ld + f] = val;
   }
 }
@@ -620,9 +616,8 @@ int nmfp_stage_a_impl(const fastfp_pack* pk, const double* d_freqs, int64_t F, d
   // stage-A tiles are written sparsely (rows of narrower pulsars, the tail of the last tile): clear
   FFP_CUDA(cudaMemsetAsync(dZ, 0, (size_t)P * nt32 * (MV * 64) * 8, st));
   FFP_CUDA(cudaMemsetAsync(dA, 0, (size_t)P * nt32 * 160 * 8, st));
-  NmfpOut nm{dZ, dA, MV};
   // on the tensor path when the pack carries digit planes, else on the fp64 DMMA kernel
-  return launch_sweep(pk, d_freqs, F, nullptr, st, &nm);
+  return launch_sweep(pk, d_freqs, F, NmfpTiles{dZ, dA, MV}, st);
 }
 
 // Factor + stage B for D draws on tiles that already exist: Z and A hold blocks of nt_blk tiles ([block][P][nt_blk]),
