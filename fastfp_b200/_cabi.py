@@ -79,6 +79,7 @@ SYMBOLS = {
     "fastfp_hash64": (C.c_uint64, [C.c_void_p, C.c_int64, C.c_uint64]),
     "fastfp_hash64_many": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "fastfp_kernel_launches": (C.c_int64, []),
+    "fastfp_device_bytes": (C.c_int64, []),
     "fastfp_xcy": (
         C.c_int,
         [C.c_int, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
@@ -550,3 +551,8 @@ def fp64_peak(kind: int = 0, iters: int = 20000, device: int = 0):
 
 def kernel_launches() -> int:
     return int(load().fastfp_kernel_launches())
+
+
+def device_bytes() -> int:
+    """Device memory the library holds now, in bytes, over all packs and devices of this process."""
+    return int(load().fastfp_device_bytes())

@@ -10,6 +10,7 @@
 namespace ffp {
 
 std::atomic<int64_t> g_launches{0};
+std::atomic<int64_t> g_device_bytes{0};
 static thread_local std::string t_err;
 
 void set_error(const std::string& msg) { t_err = msg; }
@@ -107,17 +108,18 @@ static int pack_layout(fastfp_pack* pk, int P, const int64_t* n, const int64_t* 
     groups[kc].push_back(p);
   }
   pk->mvar_total = var_off;
-  FFP_CUDA(cudaMalloc(&pk->d_meta, sizeof(PulsarMeta) * P));
-  FFP_CUDA(cudaMemcpy(pk->d_meta, pk->meta.data(), sizeof(PulsarMeta) * P, cudaMemcpyHostToDevice));
-  FFP_CUDA(cudaMalloc(&pk->d_packets, (size_t)pk_off * 8));
-  FFP_CUDA(cudaMalloc(&pk->d_L, (size_t)L_off * 8));
-  FFP_CUDA(cudaMalloc(&pk->d_info, sizeof(int) * P));
-  FFP_CUDA(cudaMemset(pk->d_info, 0, sizeof(int) * P));
+  PackCore& c = pk->core;
+  FFP_CUDA(dev_alloc(&c.meta, (size_t)P));
+  FFP_CUDA(cudaMemcpy(c.meta.get(), pk->meta.data(), sizeof(PulsarMeta) * P, cudaMemcpyHostToDevice));
+  FFP_CUDA(dev_alloc(&c.packets, (size_t)pk_off));
+  FFP_CUDA(dev_alloc(&c.L, (size_t)L_off));
+  FFP_CUDA(dev_alloc(&c.info, (size_t)P));
+  FFP_CUDA(cudaMemset(c.info.get(), 0, sizeof(int) * P));
   FFP_CUDA(cudaDeviceGetAttribute(&pk->num_sms, cudaDevAttrMultiProcessorCount, pk->device));
-  const size_t slab_bytes = (size_t)CTAS_PER_SM * pk->num_sms * sweep_max_slab_doubles() * 8;
-  FFP_CUDA(cudaMalloc(&pk->d_slab, slab_bytes));
-  FFP_CUDA(cudaMalloc(&pk->d_counter, sizeof(unsigned int)));
-  pk->bytes = pk_off * 8 + L_off * 8 + (int64_t)sizeof(PulsarMeta) * P + (int64_t)slab_bytes;
+  const size_t slab_doubles = (size_t)CTAS_PER_SM * pk->num_sms * sweep_max_slab_doubles();
+  FFP_CUDA(dev_alloc(&c.slab, slab_doubles));
+  FFP_CUDA(dev_alloc(&c.counter, 1));
+  pk->bytes = pk_off * 8 + L_off * 8 + (int64_t)sizeof(PulsarMeta) * P + (int64_t)slab_doubles * 8;
   return upload_groups(groups, &pk->groups);
 }
 
@@ -159,14 +161,7 @@ static void set_ninv_sums(fastfp_pack* pk, const double* const* Nvecs) {
 static void pack_free(fastfp_pack* pk) {
   if (!pk) return;
   DeviceGuard g(pk->device);
-  for (auto& gr : pk->groups) { cudaFree(gr.d_pidx); cudaFree(gr.d_pidx_rest); }
-  cudaFree(pk->d_meta); cudaFree(pk->d_packets); cudaFree(pk->d_L); cudaFree(pk->d_info);
-  cudaFree(pk->d_S0); cudaFree(pk->d_zr); cudaFree(pk->d_slab); cudaFree(pk->d_counter); cudaFree(pk->d_done_mask);
-  cudaFree(pk->d_pl); cudaFreeHost(pk->h_pl);
-  cudaFree(pk->d_i8); cudaFree(pk->d_i8_scale); cudaFree(pk->d_pidx_all);
-  if (pk->pl_event) cudaEventDestroy(pk->pl_event);
-  res_release(pk);
-  delete pk;  // and with it the pack's scratch, while its device is current
+  delete pk;  // the pack owns all its memory: released while its device is current
 }
 
 struct BlockNHost {  // host side arrays of a block-diagonal N (fastfp_pack_create_blockn)
@@ -181,13 +176,14 @@ static int stage_slots(fastfp_pack* pk, const BlockNHost& bn, DeviceBuf<int>* d_
   int64_t ntot = 0, nchtot = 0;
   for (auto& pm : pk->meta) { ntot += pm.n; nchtot += pm.nch; }
   FFP_CUDA(dev_alloc(d_sidx, (size_t)ntot));
-  FFP_CUDA(cudaMalloc(&pk->d_done_mask, (size_t)nchtot));
+  FFP_CUDA(dev_alloc(&pk->core.done_mask, (size_t)nchtot));
   for (int p = 0; p < pk->P; ++p) {
     const PulsarMeta& pm = pk->meta[p];
     if (!bn.slot_idx[p] || !bn.done_mask[p]) { set_error("null slot array"); return FASTFP_ERR_INVALID; }
     FFP_CUDA(cudaMemcpyAsync(d_sidx->get() + pm.raw_off, bn.slot_idx[p], (size_t)pm.n * sizeof(int),
                              cudaMemcpyHostToDevice, st));
-    FFP_CUDA(cudaMemcpyAsync(pk->d_done_mask + pm.dm_off, bn.done_mask[p], (size_t)pm.nch, cudaMemcpyHostToDevice, st));
+    FFP_CUDA(cudaMemcpyAsync(pk->core.done_mask.get() + pm.dm_off, bn.done_mask[p], (size_t)pm.nch,
+                             cudaMemcpyHostToDevice, st));
   }
   return 0;
 }
@@ -219,7 +215,7 @@ static int build_pack(int device, int P, const int64_t* n, const int64_t* m, con
   const BlockNDev* bnp = bn ? &bnd : nullptr;
   if (!rc && !bn) set_ninv_sums(pk, Nvecs);  // only the tensor sweep reads them, and it takes no block-N pack
   if (!rc && !pk->nmfp) {
-    rc = upload_ragged(pk->d_L, mats, pk, 2, st);  // sigmas, into the factor buffer pack_layout allocated
+    rc = upload_ragged(pk->core.L.get(), mats, pk, 2, st);  // sigmas, into the factor buffer pack_layout allocated
     if (!rc) rc = launch_fp_precompute(pk, d_toas.get(), d_res.get(), d_Nvec.get(), d_T.get(), st, nullptr, bnp);
     if (!rc) rc = build_i8_planes(pk, st);  // digit planes for the pulsars the tensor sweep takes (none with block-N)
   } else if (!rc) {
@@ -327,6 +323,7 @@ int fastfp_device_count(void) {
   return n;
 }
 int64_t fastfp_kernel_launches(void) { return g_launches.load(); }
+int64_t fastfp_device_bytes(void) { return g_device_bytes.load(); }
 
 int fastfp_pack_create(int device, int P, const int64_t* n, const int64_t* m,
                        const double* const* toas, const double* const* residuals,
@@ -344,12 +341,12 @@ int fastfp_pack_set_path(fastfp_pack_t* pk, int path) {
     set_error("fastfp_pack_set_path: invalid argument");
     return FASTFP_ERR_INVALID;
   }
-  if (path == FASTFP_PATH_I8 && !(pk->i8_ok && pk->i8_all())) {
+  if (path == FASTFP_PATH_I8 && !(pk->i8.ok && pk->i8_all())) {
     set_error("fastfp_pack_set_path: not every pulsar of this pack has INT8 digit planes (block-diagonal N, m > 639, "
               "n > 16384 or non-finite data); FASTFP_PATH_MIXED sweeps those on the fp64 kernel");
     return FASTFP_ERR_UNSUPPORTED;
   }
-  if (path == FASTFP_PATH_MIXED && !pk->i8_ok) {
+  if (path == FASTFP_PATH_MIXED && !pk->i8.ok) {
     set_error("fastfp_pack_set_path: no pulsar of this pack has INT8 digit planes");
     return FASTFP_ERR_UNSUPPORTED;
   }
@@ -399,7 +396,7 @@ int fastfp_pack_create_blockn(int device, int P, const int64_t* n, const int64_t
 }
 
 void fastfp_pack_destroy(fastfp_pack_t* pack) { pack_free(pack); }
-int64_t fastfp_pack_bytes(const fastfp_pack_t* pack) { return pack ? pack->bytes + pack->res_bytes : 0; }
+int64_t fastfp_pack_bytes(const fastfp_pack_t* pack) { return pack ? pack->bytes + pack->res.bytes : 0; }
 int fastfp_pack_num_pulsars(const fastfp_pack_t* pack) { return pack ? pack->P : 0; }
 int64_t fastfp_pack_mvar_total(const fastfp_pack_t* pack) { return pack ? pack->mvar_total : 0; }
 int fastfp_pack_factor_info(const fastfp_pack_t* pack, int32_t* info) {
@@ -476,7 +473,7 @@ int fastfp_pack_set_residuals(fastfp_pack_t* pk, int64_t R, const double* const*
   PackCall c(pk, stream);
   if (int rc = c.select()) return rc;
   FFP_CUDA(cudaStreamSynchronize(c.st));  // sweeps queued on this stream may still read the previous set
-  res_release(pk);
+  pk->res = {};
   if (R == 0) return FASTFP_OK;
   const int64_t n_tot = pk->meta.back().raw_off + pk->meta.back().n;
   DeviceBuf<double> d_res;
@@ -486,9 +483,7 @@ int fastfp_pack_set_residuals(fastfp_pack_t* pk, int64_t R, const double* const*
     FFP_CUDA(cudaMemcpyAsync(d_res.get() + R * pm.raw_off, residuals[p], (size_t)(R * pm.n) * 8,
                              cudaMemcpyHostToDevice, c.st));
   }
-  const int rc = build_res_packets(pk, R, d_res.get(), c.st);
-  if (rc) res_release(pk);
-  return rc;
+  return build_res_packets(pk, R, d_res.get(), c.st);
 }
 
 int fastfp_fp_sweep_residuals(const fastfp_pack_t* pk, const double* freqs, int64_t F, double* out, int flags,
@@ -497,24 +492,24 @@ int fastfp_fp_sweep_residuals(const fastfp_pack_t* pk, const double* freqs, int6
     set_error("fastfp_fp_sweep_residuals: null argument or negative F");
     return FASTFP_ERR_INVALID;
   }
-  if (pk->res_R == 0) {
+  if (pk->res.R == 0) {
     set_error("fastfp_fp_sweep_residuals: no residual realisations set (fastfp_pack_set_residuals)");
     return FASTFP_ERR_INVALID;
   }
   if (F == 0) return FASTFP_OK;
   const int P = pk->P;
-  const int64_t R = pk->res_R;
+  const int64_t R = pk->res.R;
   PackCall c(pk, stream);
   const double* d_freqs;
   double* d_out;
   if (int rc = c.stage(freqs, F, out, R * F, flags, &d_freqs, &d_out, &pk->out)) return rc;
   const int64_t FB = freq_batch(F, R * P);
-  if (int rc = pk->res_terms.grow(R * P * std::min(FB, F))) return rc;
+  if (int rc = pk->res.terms.grow(R * P * std::min(FB, F))) return rc;
   for (int64_t lo = 0; lo < F; lo += FB) {
     const int64_t fb = std::min(FB, F - lo);
-    const ResOut ro{pk->res_terms.get(), nullptr, nullptr, (int)R, P};
+    const ResOut ro{pk->res.terms.get(), nullptr, nullptr, (int)R, P};
     if (int rc = launch_fp_sweep_res(pk, d_freqs + lo, fb, ro, c.st)) return rc;
-    if (int rc = launch_reduce_terms_rows(pk->res_terms.get(), (int)R, P, fb, d_out + lo, F, c.st)) return rc;
+    if (int rc = launch_reduce_terms_rows(pk->res.terms.get(), (int)R, P, fb, d_out + lo, F, c.st)) return rc;
   }
   return c.finish(flags, R * F, out, d_out, false);
 }
@@ -571,8 +566,8 @@ int fastfp_fe_skymax(const fastfp_pack_t* pk, const double* freqs, int64_t F, co
   // weights of the S sky positions, the per-chunk bests of a split sky, and the indices on their way to host memory
   // (int64, 8 bytes per slot like the doubles). Like every scratch buffer of the pack it grows on demand and is kept
   // until the pack is destroyed: 5 P F_batch + 7 S P doubles, plus F for host outputs and a small split scratch; about
-  // 750 MB after a call with S = 196 608 and P = 68. Allocating it per call instead costs a cudaMalloc / cudaFree pair per call, measured at up
-  // to several times the whole call at C2 sizes.
+  // 750 MB after a call with S = 196 608 and P = 68. Allocating it per call instead costs a device allocation and
+  // release per call, measured at up to several times the whole call at C2 sizes.
   const int64_t n_part = plan.nchunk > 1 ? plan.nchunk * fb0 : 0;
   const bool idx_to_host = !(flags & FASTFP_OUT_ON_DEVICE);
   ScratchLayout lay;
@@ -609,14 +604,14 @@ int fastfp_fe_skymax_residuals(const fastfp_pack_t* pk, const double* freqs, int
     set_error("fastfp_fe_skymax_residuals needs a plain-Fp pack (fastfp_pack_create)");
     return FASTFP_ERR_INVALID;
   }
-  if (pk->res_R == 0) {
+  if (pk->res.R == 0) {
     set_error("fastfp_fe_skymax_residuals: no residual realisations set (fastfp_pack_set_residuals)");
     return FASTFP_ERR_INVALID;
   }
   if (F == 0) return FASTFP_OK;
   if (S == 0) { set_error("fastfp_fe_skymax_residuals needs at least one sky position"); return FASTFP_ERR_INVALID; }
   const int P = pk->P;
-  const int64_t R = pk->res_R;
+  const int64_t R = pk->res.R;
   PackCall c(pk, stream);
   const double* d_freqs;
   double* d_max;
@@ -629,7 +624,7 @@ int fastfp_fe_skymax_residuals(const fastfp_pack_t* pk, const double* freqs, int
   // of the batch, the antenna patterns, the per-chunk bests of a split sky and the indices on their way to host memory
   const int64_t n_part = plan.nchunk > 1 ? plan.nchunk * R * fb0 : 0;
   const bool idx_to_host = !(flags & FASTFP_OUT_ON_DEVICE);
-  if (int rc = pk->res_terms.grow(2 * R * P * fb0)) return rc;
+  if (int rc = pk->res.terms.grow(2 * R * P * fb0)) return rc;
   ScratchLayout lay;
   const int64_t o_mi = lay.take(3 * (int64_t)P * fb0), o_fp = lay.take(S * P), o_fx = lay.take(S * P),
                 o_part_v = lay.take(n_part), o_part_i = lay.take(n_part), o_idx = lay.take(idx_to_host ? R * F : 0);
@@ -641,9 +636,9 @@ int fastfp_fe_skymax_residuals(const fastfp_pack_t* pk, const double* freqs, int
   if (int rc = c.upload_sky(fplus, fcross, S * P, d_fp, d_fx)) return rc;
   for (int64_t lo = 0; lo < F; lo += FB) {
     const int64_t fb = std::min(FB, F - lo);
-    const ResOut ro{nullptr, pk->res_terms.get(), d_mi, (int)R, P};
+    const ResOut ro{nullptr, pk->res.terms.get(), d_mi, (int)R, P};
     if (int rc = launch_fp_sweep_res(pk, d_freqs + lo, fb, ro, c.st)) return rc;
-    if (int rc = launch_fe_skymax_res(pk->res_terms.get(), d_mi, P, R, fb, d_fp, d_fx, S, plan, part_v, part_i,
+    if (int rc = launch_fe_skymax_res(pk->res.terms.get(), d_mi, P, R, fb, d_fp, d_fx, S, plan, part_v, part_i,
                                       d_max + lo, d_idx + lo, F, c.st))
       return rc;
   }

@@ -8,7 +8,10 @@
 #include <map>
 #include <memory>
 #include <string>
+#include <type_traits>
 #include <vector>
+
+#include "../../include/fastfp_b200.h"
 
 namespace ffp {
 
@@ -110,15 +113,8 @@ struct KernelCfg {  // run-time mirror of SweepCfg's parameters
   }
 };
 
-struct Group {  // pulsars that share one kernel instantiation
-  KernelCfg cfg;
-  int count;
-  int* d_pidx;  // device array of pulsar indices
-  int count_rest = 0;          // ... those of them the tensor sweep does not take (build_i8_planes), when it takes some
-  int* d_pidx_rest = nullptr;
-};
-
 extern std::atomic<int64_t> g_launches;
+extern std::atomic<int64_t> g_device_bytes;  // device memory this library holds (fastfp_device_bytes)
 void set_error(const std::string& msg);
 int cuda_fail(cudaError_t e, const char* what);
 
@@ -128,19 +124,72 @@ int cuda_fail(cudaError_t e, const char* what);
     if (e__ != cudaSuccess) return ffp::cuda_fail(e__, #call); \
   } while (0)
 
-// device memory a host function holds for one call: cudaFree'd when the holder goes out of scope, on every return path
+// ---- owners: every allocation of the library is released by its holder, on every path -----------
+// device memory: allocated only by dev_alloc, which counts it in g_device_bytes; the deleter takes the count back
 struct CudaFree {
-  void operator()(void* p) const { cudaFree(p); }
+  size_t bytes = 0;
+  void operator()(void* p) const {
+    cudaFree(p);
+    g_device_bytes -= (int64_t)bytes;
+  }
 };
 template <typename T>
 using DeviceBuf = std::unique_ptr<T, CudaFree>;
+// count elements of T into *buf; the buffer it held before is released after the new allocation (Scratch::grow
+// releases first where the two must not coexist)
 template <typename T>
 inline cudaError_t dev_alloc(DeviceBuf<T>* buf, size_t count) {
   T* p = nullptr;
-  const cudaError_t e = cudaMalloc(&p, count * sizeof(T));
+  const size_t bytes = count * sizeof(T);
+  const cudaError_t e = cudaMalloc(&p, bytes);
+  if (e != cudaSuccess) {
+    buf->reset();
+    return e;
+  }
+  g_device_bytes += (int64_t)bytes;
+  *buf = DeviceBuf<T>(p, CudaFree{bytes});
+  return e;
+}
+// pinned host memory
+struct CudaFreeHost {
+  void operator()(void* p) const { cudaFreeHost(p); }
+};
+template <typename T>
+using PinnedBuf = std::unique_ptr<T, CudaFreeHost>;
+template <typename T>
+inline cudaError_t pinned_alloc(PinnedBuf<T>* buf, size_t count) {
+  T* p = nullptr;
+  const cudaError_t e = cudaMallocHost(&p, count * sizeof(T));
   buf->reset(e == cudaSuccess ? p : nullptr);
   return e;
 }
+// events
+struct CudaEventDestroy {
+  void operator()(cudaEvent_t e) const { cudaEventDestroy(e); }
+};
+using Event = std::unique_ptr<std::remove_pointer_t<cudaEvent_t>, CudaEventDestroy>;
+inline cudaError_t event_create(Event* ev, unsigned flags = cudaEventDefault) {
+  cudaEvent_t e = nullptr;
+  const cudaError_t rc = cudaEventCreateWithFlags(&e, flags);
+  ev->reset(rc == cudaSuccess ? e : nullptr);
+  return rc;
+}
+
+// the pulsars one sweep launch takes: a configuration and a device list of pulsar indices
+struct GroupView {
+  KernelCfg cfg;
+  const int* pidx;
+  int count;
+};
+struct Group {  // pulsars that share one kernel instantiation
+  KernelCfg cfg;
+  int count = 0;
+  DeviceBuf<int> pidx;       // their indices
+  int count_rest = 0;        // ... those of them the tensor sweep does not take (build_i8_planes), when it takes some
+  DeviceBuf<int> pidx_rest;
+  GroupView all() const { return {cfg, pidx.get(), count}; }
+  GroupView rest() const { return {cfg, pidx_rest.get(), count_rest}; }
+};
 
 // device memory a pack keeps for its calls: grown on demand (contents are not preserved), kept until released
 template <typename T>
@@ -161,6 +210,57 @@ struct Scratch {
   }
 };
 
+// ---- the memory of a pack, one owner per feature that creates it ----------------------------------
+// Releasing a feature replaces its struct with an empty one.
+
+// every pack (pack_layout; the slot masks: block-N packs, stage_slots)
+struct PackCore {
+  DeviceBuf<PulsarMeta> meta;
+  DeviceBuf<double> packets;           // [sum_p nch_p][PK_p]
+  DeviceBuf<double> L;                 // Cholesky factors (Fp) / fixed-block factors (nmfp)
+  DeviceBuf<int> info;                 // per-pulsar factorisation status
+  DeviceBuf<double> slab;              // level-2 accumulation scratch, one slab per resident CTA
+  DeviceBuf<unsigned int> counter;     // persistent-CTA work counter
+  DeviceBuf<unsigned char> done_mask;  // block-N: per-chunk epoch-slot masks
+};
+
+// INT8 tensor-core path (fp_sweep_i8.cu, build_i8_planes): digit planes of G, per-row scales
+struct TensorPath {
+  DeviceBuf<unsigned char> planes;
+  DeviceBuf<double> scale;  // [P][128]
+  DeviceBuf<int> pidx;      // pulsars on the tensor sweep (all of them, or those that fit: n <= 16384, finite planes)
+  int count = 0;            // their number; the others stay on the fp64 kernel in the same sweep
+  bool ok = false;          // the planes exist
+  int rows_max = 0;
+};
+
+// nmfp packs (nmfp_pack_finish)
+struct NmfpState {
+  DeviceBuf<double> S0;  // [P][mvpad][mvpad] Schur complement of the fixed block (no phiinv)
+  DeviceBuf<double> zr;  // [P][mvpad]  z'_r
+};
+
+// staging of the per-draw power-law parameters (fastfp_powerlaw_phiinv): device + pinned host copy of cap doubles;
+// the event marks the last H2D copy out of the host copy; tab is the frequency table already on the device
+struct PowerlawStaging {
+  DeviceBuf<double> dev;
+  PinnedBuf<double> host;
+  Event event;
+  int64_t cap = 0;
+  std::vector<double> tab;
+};
+
+// residual batch (fastfp_pack_set_residuals, DESIGN.md section 5d): per pulsar, the G rows followed by the R
+// realisations' w_k rows from row roundup8(m) on, in packets of the kernel configuration for that many rows
+struct ResidualBatch {
+  DeviceBuf<double> packets;
+  DeviceBuf<PulsarMeta> meta;
+  std::vector<Group> groups;
+  mutable Scratch<double> terms;  // [R][P][F_batch] terms of one frequency batch
+  int64_t R = 0;
+  int64_t bytes = 0;
+};
+
 }  // namespace ffp
 
 // The opaque handle of include/fastfp_b200.h.
@@ -170,36 +270,21 @@ struct fastfp_pack {
   int num_sms = 0;
   bool nmfp = false;
   bool ecorr = false;            // block-diagonal N (kernel ECORR): 8 epoch-slot rows in the G tiles
-  unsigned char* d_done_mask = nullptr;
   std::vector<ffp::PulsarMeta> meta;
   std::vector<ffp::Group> groups;
-  ffp::PulsarMeta* d_meta = nullptr;
-  double* d_packets = nullptr;  // [sum_p nch_p][PK_p]
-  double* d_L = nullptr;        // Cholesky factors (Fp) / fixed-block factors (nmfp)
-  int* d_info = nullptr;        // per-pulsar factorisation status
-  std::vector<int> info;        // host copy, read back when the pack is built (fastfp_pack_factor_info)
-  double* d_slab = nullptr;     // level-2 accumulation scratch, one slab per resident CTA
-  unsigned int* d_counter = nullptr;  // persistent-CTA work counter
-  // INT8 tensor-core path (fp_sweep_i8.cu): digit planes of G, per-row scales; chosen per pack
-  unsigned char* d_i8 = nullptr;
-  double* d_i8_scale = nullptr;   // [P][128]
-  int* d_pidx_all = nullptr;      // pulsars on the tensor sweep (all of them, or those that fit: n <= 16384, finite planes)
-  int i8_count = 0;               // their number; the others stay on the fp64 kernel in the same sweep
-  bool i8_ok = false;             // the planes exist (every pulsar fits the tile, all values finite)
-  int i8_rows_max = 0;
-  int64_t i8_bytes = 0;
-  int path = 0;                   // FASTFP_PATH_AUTO / _FP64 / _I8 / _MIXED (fastfp_pack_set_path)
+  std::vector<int> info;         // host copy of core.info, read back when the pack is built (fastfp_pack_factor_info)
+  ffp::PackCore core;
+  ffp::TensorPath i8;            // chosen per pack (path)
+  int path = 0;                  // FASTFP_PATH_AUTO / _FP64 / _I8 / _MIXED (fastfp_pack_set_path)
   // AUTO resolves to the fp64 DMMA kernel: on an H100 it sweeps m = 72 bases about twice as fast as the tensor kernel
   // (C2: 35 ms against 78 ms per step, 400 W H100 SXM). I8 and MIXED select the tensor kernel.
-  bool use_i8() const { return i8_ok && (path == 2 || path == 3); }
-  bool i8_all() const { return i8_count == P; }
+  bool use_i8() const { return i8.ok && (path == FASTFP_PATH_I8 || path == FASTFP_PATH_MIXED); }
+  bool i8_all() const { return i8.count == P; }
   int64_t bytes = 0;
   int64_t mvar_total = 0;
   int mvar_max = 0;
   int mvpad = 0;           // nmfp: per-draw block width padded to the stage-B tile (32, 64 or 96)
-  // nmfp only
-  double* d_S0 = nullptr;  // [P][mvpad][mvpad] Schur complement of the fixed block (no phiinv)
-  double* d_zr = nullptr;  // [P][mvpad]  z'_r
+  ffp::NmfpState nm;
   // scratch reused across sweeps
   mutable ffp::Scratch<double> terms;
   mutable ffp::Scratch<double> freqs;
@@ -207,21 +292,8 @@ struct fastfp_pack {
   mutable ffp::Scratch<double> scratch;  // nmfp: stage-A tiles of a frequency batch
   mutable ffp::Scratch<double> lf;       // nmfp: L^-1 fragments of a draw batch
   mutable ffp::Scratch<double> inner;    // Fe-statistic: inner products of a frequency batch + antenna patterns
-  // staging of the per-draw power-law parameters (fastfp_powerlaw_phiinv): device + pinned host copy,
-  // the event marks the last H2D copy out of h_pl; pl_tab is the frequency table already on the device
-  mutable double* d_pl = nullptr;
-  mutable double* h_pl = nullptr;
-  mutable int64_t pl_cap = 0;
-  mutable cudaEvent_t pl_event = nullptr;
-  mutable std::vector<double> pl_tab;
-  // residual batch (fastfp_pack_set_residuals, DESIGN.md section 5d): per pulsar, the G rows followed by the res_R
-  // realisations' w_k rows from row roundup8(m) on, in packets of the kernel configuration for that many rows
-  int64_t res_R = 0;
-  int64_t res_bytes = 0;
-  double* d_res_packets = nullptr;
-  ffp::PulsarMeta* d_res_meta = nullptr;
-  std::vector<ffp::Group> res_groups;
-  mutable ffp::Scratch<double> res_terms;  // [R][P][F_batch] terms of one frequency batch
+  mutable ffp::PowerlawStaging pl;
+  ffp::ResidualBatch res;
   // optional per-stage timing of nmfp sweeps (fastfp_nmfp_stage_timing): stage A, factor, stage B
   mutable bool time_stages = false;
   mutable double stage_ms[3] = {0.0, 0.0, 0.0};
@@ -240,10 +312,9 @@ int launch_fp_precompute(fastfp_pack* pk, const double* d_toas, const double* d_
                          const double* d_Nvec, const double* d_T, cudaStream_t st,
                          double* d_ur_keep = nullptr,  // [P][MAX_M], receives G r
                          const BlockNDev* bn = nullptr);
-// the residual packets of R realisations (d_res: per pulsar (R, n_p) row-major at R * raw_off); replaces any earlier
-// set. res_release frees them (R = 0).
+// the residual packets of R realisations (d_res: per pulsar (R, n_p) row-major at R * raw_off) into pk->res, which the
+// caller has released
 int build_res_packets(fastfp_pack* pk, int64_t R, const double* d_res, cudaStream_t st);
-void res_release(fastfp_pack* pk);
 // the pulsars of each kernel configuration as Groups with their indices on the device, appended to *out
 int upload_groups(const std::map<KernelCfg, std::vector<int>>& groups, std::vector<Group>* out);
 // fe.cu

@@ -35,7 +35,8 @@ __global__ void reduce_terms_kernel(const double* __restrict__ terms, int P, int
   out[f] = acc;
 }
 
-static int dispatch_group(const fastfp_pack* pk, const Group& g, const SweepArgs& a, SweepMode mode, cudaStream_t st) {
+static int dispatch_group(const fastfp_pack* pk, const GroupView& g, const SweepArgs& a, SweepMode mode,
+                          cudaStream_t st) {
   if (g.cfg.wmw == 8) return dispatch_sweep_xwide(pk, g, a, mode, st);
   if (g.cfg.wmw == 4) return dispatch_sweep_wide(pk, g, a, mode, st);
   if (g.cfg.wmw == 1 && g.cfg.nnb == 4) return dispatch_sweep_w1(pk, g, a, mode, st);
@@ -50,8 +51,8 @@ static SweepArgs sweep_args(const double* packets, const PulsarMeta* meta, const
   a.meta = meta;
   a.freqs = d_freqs;
   a.F = F;
-  a.slab = pk->d_slab;
-  a.counter = pk->d_counter;
+  a.slab = pk->core.slab.get();
+  a.counter = pk->core.counter.get();
   return a;
 }
 
@@ -61,29 +62,25 @@ static int launch_fp_groups(const fastfp_pack* pk, SweepArgs a, SweepMode mode, 
   static const int dbg = getenv("FASTFP_DBG") ? atoi(getenv("FASTFP_DBG")) : 0;
   a.dbg = dbg;
 #endif
-  a.done_mask = pk->d_done_mask;
-  for (const Group& g0 : pk->groups) {
-    Group g = g0;
-    if (rest_only) {
-      if (g0.count_rest == 0) continue;
-      g.count = g0.count_rest;
-      g.d_pidx = g0.d_pidx_rest;
-    }
-    if (int rc = dispatch_group(pk, g, a, mode, st)) return rc;
+  a.done_mask = pk->core.done_mask.get();
+  for (const Group& g : pk->groups) {
+    const GroupView v = rest_only ? g.rest() : g.all();
+    if (v.count == 0) continue;
+    if (int rc = dispatch_group(pk, v, a, mode, st)) return rc;
   }
   return 0;
 }
 
 int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, const FpOut& out, cudaStream_t st,
                     bool rest_only) {
-  SweepArgs a = sweep_args(pk->d_packets, pk->d_meta, pk, d_freqs, F);
+  SweepArgs a = sweep_args(pk->core.packets.get(), pk->core.meta.get(), pk, d_freqs, F);
   a.fp = out;
   return launch_fp_groups(pk, a, SweepMode::Fp, rest_only, st);
 }
 
 int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, const NmfpTiles& out, cudaStream_t st,
                     bool rest_only) {
-  SweepArgs a = sweep_args(pk->d_packets, pk->d_meta, pk, d_freqs, F);
+  SweepArgs a = sweep_args(pk->core.packets.get(), pk->core.meta.get(), pk, d_freqs, F);
   a.nm = out;
   return launch_fp_groups(pk, a, SweepMode::Nmfp, rest_only, st);
 }
@@ -91,10 +88,10 @@ int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, con
 // The residual batch (DESIGN.md sections 5d, 5e): the fp64 kernel on the pack's residual packets, whose G tiles carry
 // the realisations' w_k as extra rows
 int launch_fp_sweep_res(const fastfp_pack* pk, const double* d_freqs, int64_t F, const ResOut& out, cudaStream_t st) {
-  SweepArgs a = sweep_args(pk->d_res_packets, pk->d_res_meta, pk, d_freqs, F);
+  SweepArgs a = sweep_args(pk->res.packets.get(), pk->res.meta.get(), pk, d_freqs, F);
   a.res = out;
-  for (const Group& g : pk->res_groups)
-    if (int rc = dispatch_group(pk, g, a, SweepMode::Res, st)) return rc;
+  for (const Group& g : pk->res.groups)
+    if (int rc = dispatch_group(pk, g.all(), a, SweepMode::Res, st)) return rc;
   return 0;
 }
 

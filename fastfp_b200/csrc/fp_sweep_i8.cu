@@ -671,26 +671,24 @@ int run_i8_peak(int kind, int iters, double* tops, double* ms_out) {
   const size_t smem = (size_t)NPL * (128 + N) * KT + 1024;
   if (kind == 17) FFP_CUDA(cudaFuncSetAttribute(i8_peak_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   else FFP_CUDA(cudaFuncSetAttribute(i8_peak_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  cudaEvent_t e0, e1;
-  FFP_CUDA(cudaEventCreate(&e0));
-  FFP_CUDA(cudaEventCreate(&e1));
+  Event e0, e1;
+  FFP_CUDA(event_create(&e0));
+  FFP_CUDA(event_create(&e1));
   float best = 1e30f;
   for (int rep = 0; rep < 4; ++rep) {
-    FFP_CUDA(cudaEventRecord(e0));
+    FFP_CUDA(cudaEventRecord(e0.get()));
     if (kind == 17) i8_peak_kernel<256><<<sms, 256, smem>>>(iters, nullptr);
     else i8_peak_kernel<32><<<sms, 256, smem>>>(iters, nullptr);
-    FFP_CUDA(cudaEventRecord(e1));
-    FFP_CUDA(cudaEventSynchronize(e1));
+    FFP_CUDA(cudaEventRecord(e1.get()));
+    FFP_CUDA(cudaEventSynchronize(e1.get()));
     float ms = 0;
-    FFP_CUDA(cudaEventElapsedTime(&ms, e0, e1));
+    FFP_CUDA(cudaEventElapsedTime(&ms, e0.get(), e1.get()));
     if (rep > 0 && ms < best) best = ms;
   }
   g_launches += 4;
   FFP_CUDA(cudaGetLastError());
   *tops = 2.0 * (double)sms * iters * 28.0 * 128.0 * N * 32.0 / (best * 1e-3) / 1e12;
   *ms_out = best;
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
   return 0;
 }
 
@@ -709,10 +707,9 @@ bool i8_eligible(const fastfp_pack* pk) {
   return false;
 }
 
-// lay out and build the digit planes from the fp64 packets (after launch_fp_precompute); sets pk->i8_ok
+// lay out and build the digit planes from the fp64 packets (after launch_fp_precompute) into pk->i8, which stays empty
+// when no pulsar can take them
 int build_i8_planes(fastfp_pack* pk, cudaStream_t st) {
-  pk->i8_ok = false;
-  pk->i8_count = 0;
   if (!i8_eligible(pk)) return 0;
   const int P = pk->P;
   int64_t off = 0;
@@ -731,19 +728,22 @@ int build_i8_planes(fastfp_pack* pk, cudaStream_t st) {
     rows_max = pm.i8_rows > rows_max ? pm.i8_rows : rows_max;
     nst_max = pm.i8_nst > nst_max ? pm.i8_nst : nst_max;
   }
-  FFP_CUDA(cudaMemcpyAsync(pk->d_meta, pk->meta.data(), sizeof(PulsarMeta) * P, cudaMemcpyHostToDevice, st));
+  const PackCore& c = pk->core;
+  FFP_CUDA(cudaMemcpyAsync(c.meta.get(), pk->meta.data(), sizeof(PulsarMeta) * P, cudaMemcpyHostToDevice, st));
+  TensorPath tp;
   // the last plane of the last stage is read 128 rows deep by the MMA only from shared memory; the global buffer
   // needs no slack, but keep the allocation 16-byte granular for the bulk copies
-  FFP_CUDA(cudaMalloc(&pk->d_i8, (size_t)off + 16));
-  FFP_CUDA(cudaMalloc(&pk->d_i8_scale, (size_t)P * i8::RS * sizeof(double)));
-  FFP_CUDA(cudaMemsetAsync(pk->d_i8_scale, 0, (size_t)P * i8::RS * sizeof(double), st));
+  FFP_CUDA(dev_alloc(&tp.planes, (size_t)off + 16));
+  FFP_CUDA(dev_alloc(&tp.scale, (size_t)P * i8::RS));
+  FFP_CUDA(cudaMemsetAsync(tp.scale.get(), 0, (size_t)P * i8::RS * sizeof(double), st));
   DeviceBuf<int> d_exp, d_bad;
   FFP_CUDA(dev_alloc(&d_exp, (size_t)P * i8::RS));
   FFP_CUDA(dev_alloc(&d_bad, (size_t)P));
   FFP_CUDA(cudaMemsetAsync(d_bad.get(), 0, (size_t)P * sizeof(int), st));
-  i8::i8_rowscale_kernel<<<dim3(rows_max, P), 256, 0, st>>>(pk->d_packets, pk->d_meta, pk->d_i8_scale, d_exp.get(),
-                                                            d_bad.get());
-  i8::i8_planes_kernel<<<dim3(nst_max, P), 256, 0, st>>>(pk->d_packets, pk->d_meta, d_exp.get(), pk->d_i8);
+  i8::i8_rowscale_kernel<<<dim3(rows_max, P), 256, 0, st>>>(c.packets.get(), c.meta.get(), tp.scale.get(),
+                                                            d_exp.get(), d_bad.get());
+  i8::i8_planes_kernel<<<dim3(nst_max, P), 256, 0, st>>>(c.packets.get(), c.meta.get(), d_exp.get(),
+                                                         tp.planes.get());
   g_launches += 2;
   cudaError_t e = cudaGetLastError();
   std::vector<int> bad(P, 0);
@@ -756,34 +756,26 @@ int build_i8_planes(fastfp_pack* pk, cudaStream_t st) {
     const bool ok = pk->meta[p].i8_nst > 0 && bad[p] == 0 && (p >= (int)pk->info.size() || pk->info[p] == 0);
     if (ok) { take.push_back(p); rest_flag[p] = 0; }
   }
-  pk->i8_rows_max = rows_max;
-  pk->i8_bytes = off;
-  if (take.empty()) {
-    cudaFree(pk->d_i8); cudaFree(pk->d_i8_scale);
-    pk->d_i8 = nullptr; pk->d_i8_scale = nullptr;
-    return 0;
-  }
-  cudaFree(pk->d_pidx_all);
-  pk->d_pidx_all = nullptr;
-  FFP_CUDA(cudaMalloc(&pk->d_pidx_all, sizeof(int) * take.size()));
-  FFP_CUDA(cudaMemcpy(pk->d_pidx_all, take.data(), sizeof(int) * take.size(), cudaMemcpyHostToDevice));
-  pk->i8_count = (int)take.size();
+  if (take.empty()) return 0;
+  FFP_CUDA(dev_alloc(&tp.pidx, take.size()));
+  FFP_CUDA(cudaMemcpy(tp.pidx.get(), take.data(), sizeof(int) * take.size(), cudaMemcpyHostToDevice));
+  tp.count = (int)take.size();
   // the complement, per kernel family of the fp64 sweep
   for (Group& g : pk->groups) {
     std::vector<int> all((size_t)g.count), rest;
-    FFP_CUDA(cudaMemcpy(all.data(), g.d_pidx, sizeof(int) * g.count, cudaMemcpyDeviceToHost));
+    FFP_CUDA(cudaMemcpy(all.data(), g.pidx.get(), sizeof(int) * g.count, cudaMemcpyDeviceToHost));
     for (int p : all)
       if (rest_flag[p]) rest.push_back(p);
-    cudaFree(g.d_pidx_rest);
-    g.d_pidx_rest = nullptr;
     g.count_rest = (int)rest.size();
     if (g.count_rest) {
-      FFP_CUDA(cudaMalloc(&g.d_pidx_rest, sizeof(int) * rest.size()));
-      FFP_CUDA(cudaMemcpy(g.d_pidx_rest, rest.data(), sizeof(int) * rest.size(), cudaMemcpyHostToDevice));
+      FFP_CUDA(dev_alloc(&g.pidx_rest, rest.size()));
+      FFP_CUDA(cudaMemcpy(g.pidx_rest.get(), rest.data(), sizeof(int) * rest.size(), cudaMemcpyHostToDevice));
     }
   }
   pk->bytes += off + (int64_t)P * i8::RS * 8;
-  pk->i8_ok = true;
+  tp.rows_max = rows_max;
+  tp.ok = true;
+  pk->i8 = std::move(tp);
   return 0;
 }
 
@@ -796,16 +788,16 @@ static int launch_i8(const fastfp_pack* pk, const double* d_freqs, int64_t F, co
   a.F = F;
   if (fp) a.fp = *fp;
   if (nm) a.nm = *nm;
-  a.planes = pk->d_i8;
-  a.rowscale = pk->d_i8_scale;
-  a.meta = pk->d_meta;
-  a.pidx = pk->d_pidx_all;
-  const int64_t ntile = (a.F + NF - 1) / NF, nwork = ntile * pk->i8_count;  // the pulsars this kernel takes
+  a.planes = pk->i8.planes.get();
+  a.rowscale = pk->i8.scale.get();
+  a.meta = pk->core.meta.get();
+  a.pidx = pk->i8.pidx.get();
+  const int64_t ntile = (a.F + NF - 1) / NF, nwork = ntile * pk->i8.count;  // the pulsars this kernel takes
   if (nwork > 0x7fffffffLL) { set_error("frequency batch too large for one launch"); return -1; }
   a.ntile = (int)ntile;
   a.nwork = (int)nwork;
   a.nt32 = (int)((a.F + 31) / 32);
-  a.gslot = NPL * (pk->i8_rows_max < 128 ? pk->i8_rows_max : 128) * KT;  // one row group
+  a.gslot = NPL * (pk->i8.rows_max < 128 ? pk->i8.rows_max : 128) * KT;  // one row group
   const size_t budget = 220 * 1024 - SMEM_FIXED;
   int gst = (int)(budget / a.gslot);
   gst = gst > 8 ? 8 : gst;

@@ -555,7 +555,7 @@ __global__ void __launch_bounds__(C::NTHREADS, CTAS_PER_SM) fp_sweep_kernel(cons
 
 // ---- launch helpers -------------------------------------------------------------------------
 template <class C, SweepMode MODE, bool ECORR>
-int launch_sweep_cfg(const fastfp_pack* pk, const Group& g, const SweepArgs& base, cudaStream_t st) {
+int launch_sweep_cfg(const fastfp_pack* pk, const GroupView& g, const SweepArgs& base, cudaStream_t st) {
   static bool attr_done[64] = {};
   if (!attr_done[pk->device & 63]) {
     FFP_CUDA(cudaFuncSetAttribute(fp_sweep_kernel<C, MODE, ECORR>,
@@ -563,7 +563,7 @@ int launch_sweep_cfg(const fastfp_pack* pk, const Group& g, const SweepArgs& bas
     attr_done[pk->device & 63] = true;
   }
   SweepArgs a = base;
-  a.pidx = g.d_pidx;
+  a.pidx = g.pidx;
   const int64_t ntile = (a.F + C::KF - 1) / C::KF;
   const int64_t nwork = ntile * g.count;
   if (nwork > 0x7fffffffLL) { set_error("frequency batch too large for one launch"); return -1; }
@@ -579,11 +579,11 @@ int launch_sweep_cfg(const fastfp_pack* pk, const Group& g, const SweepArgs& bas
 }
 
 // one translation unit per configuration family instantiates these (compile time)
-int dispatch_sweep_w1(const fastfp_pack*, const Group&, const SweepArgs&, SweepMode, cudaStream_t);
-int dispatch_sweep_w2(const fastfp_pack*, const Group&, const SweepArgs&, SweepMode, cudaStream_t);
-int dispatch_sweep_w4(const fastfp_pack*, const Group&, const SweepArgs&, SweepMode, cudaStream_t);
-int dispatch_sweep_wide(const fastfp_pack*, const Group&, const SweepArgs&, SweepMode, cudaStream_t);
-int dispatch_sweep_xwide(const fastfp_pack*, const Group&, const SweepArgs&, SweepMode, cudaStream_t);
+int dispatch_sweep_w1(const fastfp_pack*, const GroupView&, const SweepArgs&, SweepMode, cudaStream_t);
+int dispatch_sweep_w2(const fastfp_pack*, const GroupView&, const SweepArgs&, SweepMode, cudaStream_t);
+int dispatch_sweep_w4(const fastfp_pack*, const GroupView&, const SweepArgs&, SweepMode, cudaStream_t);
+int dispatch_sweep_wide(const fastfp_pack*, const GroupView&, const SweepArgs&, SweepMode, cudaStream_t);
+int dispatch_sweep_xwide(const fastfp_pack*, const GroupView&, const SweepArgs&, SweepMode, cudaStream_t);
 
 // five kernels per configuration: Fp and Nmfp, each with diagonal or block-diagonal N (pk->ecorr), and Res (diagonal N,
 // plain-Fp packs only)

@@ -402,17 +402,20 @@ int run_fp64_peak(int kind, int iters, double* tflops, double* ms_out) {
   int dev = 0, sms = 0;
   FFP_CUDA(cudaGetDevice(&dev));
   FFP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  double* sink = nullptr;
-  FFP_CUDA(cudaMalloc(&sink, 8));
-  cudaEvent_t e0, e1;
-  FFP_CUDA(cudaEventCreate(&e0));
-  FFP_CUDA(cudaEventCreate(&e1));
+  DeviceBuf<double> sink_buf;
+  FFP_CUDA(dev_alloc(&sink_buf, 1));
+  double* sink = sink_buf.get();
+  Event ev0, ev1;
+  FFP_CUDA(event_create(&ev0));
+  FFP_CUDA(event_create(&ev1));
+  cudaEvent_t e0 = ev0.get(), e1 = ev1.get();
   const int grid = sms * 8;
   float best = 1e30f;
   if (kind >= 5 && kind <= 8) {
-    long long* dc = nullptr;
+    DeviceBuf<long long> dc_buf;
+    FFP_CUDA(dev_alloc(&dc_buf, 1));
+    long long* dc = dc_buf.get();
     long long hc = 0;
-    FFP_CUDA(cudaMalloc(&dc, 8));
     for (int rep = 0; rep < 2; ++rep) {
       FFP_CUDA(cudaEventRecord(e0));
       if (kind == 5) dfma_latency_kernel<<<sms, 128>>>(iters, 1.0, sink, dc);
@@ -428,7 +431,6 @@ int run_fp64_peak(int kind, int iters, double* tflops, double* ms_out) {
     const double per = kind == 5 ? 16.0 * iters : (kind == 6 ? 1.0 : kind == 7 ? 2.0 : 4.0) * iters;
     *tflops = (double)hc / per;
     *ms_out = best;
-    cudaFree(dc); cudaEventDestroy(e0); cudaEventDestroy(e1); cudaFree(sink);
     return 0;
   }
   for (int rep = 0; rep < 4; ++rep) {
@@ -480,9 +482,6 @@ int run_fp64_peak(int kind, int iters, double* tflops, double* ms_out) {
                                        : (double)sms * 2 * 128 * 144.0 * iters;
   *tflops = 2.0 * fma_count / (best * 1e-3) / 1e12;
   *ms_out = best;
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  cudaFree(sink);
   return 0;
 }
 

@@ -85,18 +85,20 @@ int nmfp_pack_finish(fastfp_pack* pk, const double* d_toas, const double* d_res,
   const int nmbv = pk->mvar_max <= 32 ? 4 : pk->mvar_max <= 64 ? 8 : pk->mvar_max <= 96 ? 12 : pk->mvar_max <= 128 ? 16 : 0;
   if (!nmbv) { set_error("nmfp pack: more than 128 per-draw columns (64 Fourier components) is not supported"); return FASTFP_ERR_UNSUPPORTED; }
   pk->mvpad = 8 * nmbv;
-  nmfp_init_sigma_kernel<<<P, 256, 0, st>>>(pk->d_L, pk->d_meta, d_TNT, d_phiinv_fix);
+  const PackCore& c = pk->core;
+  nmfp_init_sigma_kernel<<<P, 256, 0, st>>>(c.L.get(), c.meta.get(), d_TNT, d_phiinv_fix);
   g_launches += 1;
   DeviceBuf<double> d_ur;
   FFP_CUDA(dev_alloc(&d_ur, (size_t)P * MAX_M));
   int rc = launch_fp_precompute(pk, d_toas, d_res, d_Nvec, d_T, st, d_ur.get(), bn);
   if (!rc) {
-    cudaError_t e = cudaMalloc(&pk->d_S0, (size_t)P * pk->mvpad * pk->mvpad * 8);
-    if (e == cudaSuccess) e = cudaMalloc(&pk->d_zr, (size_t)P * pk->mvpad * 8);
+    cudaError_t e = dev_alloc(&pk->nm.S0, (size_t)P * pk->mvpad * pk->mvpad);
+    if (e == cudaSuccess) e = dev_alloc(&pk->nm.zr, (size_t)P * pk->mvpad);
     if (e != cudaSuccess) rc = cuda_fail(e, "nmfp pack allocation");
   }
   if (!rc) {
-    nmfp_extract_kernel<<<P, 256, 0, st>>>(pk->d_L, pk->d_meta, d_ur.get(), pk->d_S0, pk->d_zr, pk->mvpad);
+    nmfp_extract_kernel<<<P, 256, 0, st>>>(c.L.get(), c.meta.get(), d_ur.get(), pk->nm.S0.get(), pk->nm.zr.get(),
+                                           pk->mvpad);
     g_launches += 1;
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
@@ -169,25 +171,25 @@ int powerlaw_phiinv_impl(const fastfp_pack* pk, const double* const* Ffreqs, con
     host_df(curn_Ffreqs, (int)ncurn, tmp);
     for (int64_t k = 0; k < ncurn; ++k) { tab[2 * ld + k] = curn_Ffreqs[k]; tab[2 * ld + ncurn + k] = tmp[k]; }
   }
-  if ((int64_t)(ntab + npar) > pk->pl_cap) {
-    if (pk->pl_event) cudaEventSynchronize(pk->pl_event);
-    cudaFree(pk->d_pl); cudaFreeHost(pk->h_pl);
-    pk->d_pl = pk->h_pl = nullptr; pk->pl_cap = 0; pk->pl_tab.clear();
-    FFP_CUDA(cudaMalloc(&pk->d_pl, (ntab + npar) * 8));
-    FFP_CUDA(cudaMallocHost(&pk->h_pl, (ntab + npar) * 8));
-    pk->pl_cap = (int64_t)(ntab + npar);
-    if (!pk->pl_event) FFP_CUDA(cudaEventCreateWithFlags(&pk->pl_event, cudaEventDisableTiming));
-  } else if (pk->pl_event) {
-    FFP_CUDA(cudaEventSynchronize(pk->pl_event));  // the previous call's copies have left the staging buffer
+  PowerlawStaging& pl = pk->pl;
+  if ((int64_t)(ntab + npar) > pl.cap) {
+    if (pl.event) cudaEventSynchronize(pl.event.get());
+    pl = {};
+    FFP_CUDA(dev_alloc(&pl.dev, ntab + npar));
+    FFP_CUDA(pinned_alloc(&pl.host, ntab + npar));
+    FFP_CUDA(event_create(&pl.event, cudaEventDisableTiming));
+    pl.cap = (int64_t)(ntab + npar);
+  } else {
+    FFP_CUDA(cudaEventSynchronize(pl.event.get()));  // the previous call's copies have left the staging buffer
   }
-  double* dT = pk->d_pl;
+  double* dT = pl.dev.get();
   double* dP = dT + ntab;
-  double* hT = pk->h_pl;
+  double* hT = pl.host.get();
   double* hP = hT + ntab;
-  if (pk->pl_tab != tab) {
+  if (pl.tab != tab) {
     std::copy(tab.begin(), tab.end(), hT);
     FFP_CUDA(cudaMemcpyAsync(dT, hT, ntab * 8, cudaMemcpyHostToDevice, st));
-    pk->pl_tab = tab;
+    pl.tab = tab;
   }
   std::copy(log10_A, log10_A + nA, hP);
   std::copy(gamma, gamma + nA, hP + nA);
@@ -196,11 +198,11 @@ int powerlaw_phiinv_impl(const fastfp_pack* pk, const double* const* Ffreqs, con
     std::copy(curn_gamma, curn_gamma + D, hP + 2 * nA + D);
   }
   FFP_CUDA(cudaMemcpyAsync(dP, hP, npar * 8, cudaMemcpyHostToDevice, st));
-  FFP_CUDA(cudaEventRecord(pk->pl_event, st));
+  FFP_CUDA(cudaEventRecord(pl.event.get(), st));
   const double *dF = dT, *dDf = dT + ld, *dcF = dT + 2 * ld, *dcdf = dcF + ncurn;
   const double *dA = dP, *dG = dP + nA, *dcA = dP + 2 * nA, *dcG = dcA + D;
   dim3 grid((unsigned)D, P);
-  powerlaw_phiinv_kernel<<<grid, 64, 0, st>>>(pk->d_meta, dF, dDf, dA, dG, P, dcF, dcdf, (int)ncurn, dcA, dcG,
+  powerlaw_phiinv_kernel<<<grid, 64, 0, st>>>(pk->core.meta.get(), dF, dDf, dA, dG, P, dcF, dcdf, (int)ncurn, dcA, dcG,
                                                out, ld);
   g_launches += 1;
   FFP_CUDA(cudaGetLastError());
@@ -562,13 +564,13 @@ __global__ void __launch_bounds__(StageBCfg<NMBV>::THREADS, 1) nmfp_stageB_kerne
 // ending at a mark is charged to that mark's stage (0 = stage A incl. clears, 1 = factor, 2 = stage B).
 struct StageMarks {
   bool on = false;
-  std::vector<std::pair<cudaEvent_t, int>> ev;
+  std::vector<std::pair<Event, int>> ev;
   void mark(int stage, cudaStream_t st) {
     if (!on) return;
-    cudaEvent_t e;
-    if (cudaEventCreate(&e) != cudaSuccess) return;
-    cudaEventRecord(e, st);
-    ev.push_back({e, stage});
+    Event e;
+    if (event_create(&e) != cudaSuccess) return;
+    cudaEventRecord(e.get(), st);
+    ev.emplace_back(std::move(e), stage);
   }
   void finish(cudaStream_t st, double* ms3) {
     if (!on) return;
@@ -576,10 +578,9 @@ struct StageMarks {
     ms3[0] = ms3[1] = ms3[2] = 0.0;
     for (size_t i = 1; i < ev.size(); ++i) {
       float t = 0.f;
-      if (ev[i].second >= 0 && cudaEventElapsedTime(&t, ev[i - 1].first, ev[i].first) == cudaSuccess)
+      if (ev[i].second >= 0 && cudaEventElapsedTime(&t, ev[i - 1].first.get(), ev[i].first.get()) == cudaSuccess)
         ms3[ev[i].second] += t;
     }
-    for (auto& e : ev) cudaEventDestroy(e.first);
     ev.clear();
   }
 };
@@ -598,8 +599,8 @@ static int run_factor_and_stageB(const fastfp_pack* pk, const double* d_phiinv, 
   }
   constexpr int FW = FactorCfg<NMBV>::FW;
   const unsigned gf = (unsigned)(((int64_t)pk->P * Db + FW - 1) / FW);
-  nmfp_factor_kernel<NMBV><<<gf, FW * 32, fsm, st>>>(pk->d_S0, pk->d_zr, pk->d_meta, d_phiinv, ld, d_lf, sb.lfw,
-                                                   pk->P, Db);
+  nmfp_factor_kernel<NMBV><<<gf, FW * 32, fsm, st>>>(pk->nm.S0.get(), pk->nm.zr.get(), pk->core.meta.get(), d_phiinv,
+                                                   ld, d_lf, sb.lfw, pk->P, Db);
   marks.mark(1, st);
   dim3 gb((sb.nt32 + StageBCfg<NMBV>::NH - 1) / StageBCfg<NMBV>::NH, (Db + NB_DT - 1) / NB_DT);
   nmfp_stageB_kernel<NMBV><<<gb, StageBCfg<NMBV>::THREADS, bsm, st>>>(sb);
@@ -654,7 +655,8 @@ int nmfp_stage_b_impl(const fastfp_pack* pk, const double* d_freqs, int64_t F, c
   double* dLf = pk->lf.get();
   for (int64_t dd = 0; dd < D; dd += DB) {
     const int Db = (int)std::min(DB, D - dd);
-    StageBArgs sb{dZ, dA, dLf, d_freqs, pk->d_meta, d_out + dd * out_ld, F, out_ld, P, nt32, Db, lfw, nt_blk};
+    StageBArgs sb{dZ, dA, dLf, d_freqs, pk->core.meta.get(), d_out + dd * out_ld, F, out_ld, P, nt32, Db, lfw,
+                  nt_blk};
     const double* ph = d_phiinv_var + dd * pk->mvar_total;
     int rc;
     if (NMBV == 4) rc = run_factor_and_stageB<4>(pk, ph, pk->mvar_total, Db, sb, dLf, st, marks);

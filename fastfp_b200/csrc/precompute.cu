@@ -155,13 +155,14 @@ int launch_fp_precompute(fastfp_pack* pk, const double* d_toas, const double* d_
     FFP_CUDA(dev_alloc(&ur_tmp, (size_t)P * MAX_M));
     d_ur = ur_tmp.get();
   }
-  chol_kernel<<<P, 256, 0, st>>>(pk->d_L, pk->d_meta, pk->d_info);
+  const PackCore& c = pk->core;
+  chol_kernel<<<P, 256, 0, st>>>(c.L.get(), c.meta.get(), c.info.get());
   dim3 g1((nmax + 127) / 128, P);
-  build_packets_kernel<<<g1, 128, 0, st>>>(pk->d_packets, pk->d_meta, pk->d_L, d_toas, d_Nvec, d_T,
+  build_packets_kernel<<<g1, 128, 0, st>>>(c.packets.get(), c.meta.get(), c.L.get(), d_toas, d_Nvec, d_T,
                                            bn ? bn->slot_idx : nullptr, bn ? bn->slot_val : nullptr);
-  ur_kernel<<<P, 256, 0, st>>>(pk->d_packets, pk->d_meta, d_res, d_ur);
+  ur_kernel<<<P, 256, 0, st>>>(c.packets.get(), c.meta.get(), d_res, d_ur);
   // with a block-diagonal N the first term of w is N^-1 r, supplied as (N^-1 r) * Nvec
-  w_kernel<<<g1, 128, 0, st>>>(pk->d_packets, pk->d_meta, bn ? bn->res_w : d_res, d_ur);
+  w_kernel<<<g1, 128, 0, st>>>(c.packets.get(), c.meta.get(), bn ? bn->res_w : d_res, d_ur);
   g_launches += 4;
   FFP_CUDA(cudaGetLastError());
   FFP_CUDA(cudaStreamSynchronize(st));
@@ -169,7 +170,7 @@ int launch_fp_precompute(fastfp_pack* pk, const double* d_toas, const double* d_
   // SPD; the factor then carries NaN, which propagates like the reference's non-raising solve -- but the
   // caller can ask which pulsar it was (fastfp_pack_factor_info; the Python mirror warns)
   pk->info.assign(P, 0);
-  FFP_CUDA(cudaMemcpy(pk->info.data(), pk->d_info, sizeof(int) * P, cudaMemcpyDeviceToHost));
+  FFP_CUDA(cudaMemcpy(pk->info.data(), c.info.get(), sizeof(int) * P, cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -278,23 +279,11 @@ int upload_groups(const std::map<KernelCfg, std::vector<int>>& groups, std::vect
     Group g;
     g.cfg = kv.first;
     g.count = (int)kv.second.size();
-    FFP_CUDA(cudaMalloc(&g.d_pidx, sizeof(int) * g.count));
-    out->push_back(g);  // before the copy, so that the owner frees it if the copy fails
-    FFP_CUDA(cudaMemcpy(g.d_pidx, kv.second.data(), sizeof(int) * g.count, cudaMemcpyHostToDevice));
+    FFP_CUDA(dev_alloc(&g.pidx, (size_t)g.count));
+    FFP_CUDA(cudaMemcpy(g.pidx.get(), kv.second.data(), sizeof(int) * g.count, cudaMemcpyHostToDevice));
+    out->push_back(std::move(g));
   }
   return 0;
-}
-
-void res_release(fastfp_pack* pk) {
-  for (auto& g : pk->res_groups) cudaFree(g.d_pidx);
-  pk->res_groups.clear();
-  cudaFree(pk->d_res_packets);
-  cudaFree(pk->d_res_meta);
-  pk->d_res_packets = nullptr;
-  pk->d_res_meta = nullptr;
-  pk->res_terms.release();
-  pk->res_R = 0;
-  pk->res_bytes = 0;
 }
 
 int build_res_packets(fastfp_pack* pk, int64_t R, const double* d_res, cudaStream_t st) {
@@ -320,23 +309,26 @@ int build_res_packets(fastfp_pack* pk, int64_t R, const double* d_res, cudaStrea
     nmax = std::max(nmax, rm.n);
     npad = std::max(npad, rm.nch * rm.ci);
   }
-  FFP_CUDA(cudaMalloc(&pk->d_res_meta, sizeof(PulsarMeta) * P));
-  FFP_CUDA(cudaMemcpy(pk->d_res_meta, rmeta.data(), sizeof(PulsarMeta) * P, cudaMemcpyHostToDevice));
-  FFP_CUDA(cudaMalloc(&pk->d_res_packets, (size_t)off * 8));
-  if (int rc = upload_groups(groups, &pk->res_groups)) return rc;
-  pk->res_bytes = off * 8 + (int64_t)sizeof(PulsarMeta) * P;
+  ResidualBatch rb;
+  FFP_CUDA(dev_alloc(&rb.meta, (size_t)P));
+  FFP_CUDA(cudaMemcpy(rb.meta.get(), rmeta.data(), sizeof(PulsarMeta) * P, cudaMemcpyHostToDevice));
+  FFP_CUDA(dev_alloc(&rb.packets, (size_t)off));
+  if (int rc = upload_groups(groups, &rb.groups)) return rc;
+  rb.bytes = off * 8 + (int64_t)sizeof(PulsarMeta) * P;
   DeviceBuf<double> U;
   FFP_CUDA(dev_alloc(&U, (size_t)P * R * mmax));
-  res_packets_kernel<<<dim3((npad + 127) / 128, P), 128, 0, st>>>(pk->d_res_packets, pk->d_res_meta, pk->d_packets,
-                                                                  pk->d_meta);
-  ur_batch_kernel<<<dim3((mmax + 7) / 8, (unsigned)((R + 31) / 32), P), 256, 0, st>>>(pk->d_packets, pk->d_meta, d_res,
-                                                                                     (int)R, mmax, U.get());
+  const PackCore& c = pk->core;
+  res_packets_kernel<<<dim3((npad + 127) / 128, P), 128, 0, st>>>(rb.packets.get(), rb.meta.get(), c.packets.get(),
+                                                                  c.meta.get());
+  ur_batch_kernel<<<dim3((mmax + 7) / 8, (unsigned)((R + 31) / 32), P), 256, 0, st>>>(c.packets.get(), c.meta.get(),
+                                                                                     d_res, (int)R, mmax, U.get());
   w_batch_kernel<<<dim3((nmax + 31) / 32, (unsigned)((R + 7) / 8), P), 256, 0, st>>>(
-      pk->d_res_packets, pk->d_res_meta, pk->d_packets, pk->d_meta, d_res, (int)R, mmax, U.get());
+      rb.packets.get(), rb.meta.get(), c.packets.get(), c.meta.get(), d_res, (int)R, mmax, U.get());
   g_launches += 3;
   FFP_CUDA(cudaGetLastError());
   FFP_CUDA(cudaStreamSynchronize(st));  // U and the caller's staging buffer are released on return
-  pk->res_R = R;
+  rb.R = R;
+  pk->res = std::move(rb);
   return 0;
 }
 

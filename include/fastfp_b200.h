@@ -258,6 +258,7 @@ uint64_t fastfp_hash64(const void* data, int64_t nbytes, uint64_t seed);
  * buffers share one set of threads, so a list of many medium-sized arrays hashes at memory bandwidth. */
 int fastfp_hash64_many(const void* const* ptrs, const int64_t* nbytes, int32_t n, const uint64_t* seeds, uint64_t* out);
 int64_t fastfp_kernel_launches(void); /* kernels launched by this library so far (process-wide) */
+int64_t fastfp_device_bytes(void);    /* device memory this library holds now, in bytes (process-wide) */
 /* measurement aid: with enable != 0 every later fastfp_nmfp_sweep on this pack brackets its three
  * stages with CUDA events on the caller's stream and synchronises at the end; fastfp_nmfp_stage_ms
  * then returns the milliseconds of the last sweep {stage A sweep kernel + clears, per-draw factor

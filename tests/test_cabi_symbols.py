@@ -32,6 +32,9 @@ def test_library_answers_metadata_calls_without_a_gpu():
     assert lib.fastfp_version() >= 100
     assert lib.fastfp_device_count() >= 0
     assert lib.fastfp_kernel_launches() >= 0
+    assert lib.fastfp_device_bytes() >= 0
+    if lib.fastfp_device_count() == 0:  # with a device, packs of earlier tests may still be cached
+        assert lib.fastfp_device_bytes() == 0
     assert lib.fastfp_pack_bytes(None) == 0 and lib.fastfp_pack_num_pulsars(None) == 0
 
 
