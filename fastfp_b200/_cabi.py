@@ -39,6 +39,11 @@ SYMBOLS = {
     "fastfp_fe_skymax": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
                                    C.c_void_p, C.c_int, C.c_void_p]),
     "fastfp_pack_set_residuals": (C.c_int, [C.c_void_p, C.c_int64, c_double_pp, C.c_void_p]),
+    "fastfp_pack_set_residuals_blockn": (
+        C.c_int,
+        [C.c_void_p, C.c_int64, c_int64_p, c_double_pp, c_double_pp, C.POINTER(C.POINTER(C.c_int32)), c_double_pp,
+         C.POINTER(C.POINTER(C.c_ubyte)), C.c_void_p],
+    ),
     "fastfp_fp_sweep_residuals": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p]),
     "fastfp_fe_skymax_residuals": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
                                              C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
@@ -103,10 +108,11 @@ SYMBOLS = {
 MAX_M = 640  # G rows of the widest sweep kernel (csrc/ffp_internal.cuh)
 
 
-def max_residual_rows(m) -> int:
+def max_residual_rows(m, blockn: bool = False) -> int:
     """Most residual realisations ``fastfp_pack_set_residuals`` takes for pulsars of basis widths ``m``: every pulsar
-    needs ``roundup8(m_p) + roundup8(R)`` of the sweep kernel's ``MAX_M`` G rows."""
-    return MAX_M - -(-max(m) // 8) * 8
+    needs ``roundup8(m_p) + roundup8(R)`` of the sweep kernel's ``MAX_M`` G rows. A block-diagonal N pack
+    (``fastfp_pack_set_residuals_blockn``) needs 8 more, the epoch slots."""
+    return MAX_M - -(-max(m) // 8) * 8 - (8 if blockn else 0)
 
 
 class FastFpError(RuntimeError):
@@ -228,6 +234,7 @@ class Pack:
 
     PATHS = {"auto": 0, "fp64": 1, "i8": 2, "mixed": 3}
     blockn = False  # a block-diagonal N (set by create)
+    epochs = None   # block-N packs: each pulsar's blockn.Epochs (its realisations are laid out with them)
     R = 0           # realisations set by set_residuals
 
     def set_path(self, path: str) -> None:
@@ -274,7 +281,7 @@ class Pack:
             if P < 1 or not (len(residuals) == len(Nvecs) == len(Ts) == len(mats) == P):
                 raise ValueError("toas, residuals, Nvecs, Ts and the matrices must be lists of equal length P >= 1")
             Ts, mats = [as_f64(T) for T in Ts], [as_f64(a) for a in mats]
-            prep, n, m = [], [], []
+            prep, n, m, epochs = [], [], [], []
             for p in range(P):
                 if Ts[p].ndim != 2 or mats[p].shape != (Ts[p].shape[1],) * 2:
                     raise ValueError(f"pulsar {p}: Ts must be (ntoa, nbasis) and the matrix (nbasis, nbasis)")
@@ -282,6 +289,7 @@ class Pack:
                 if ci <= 0:
                     raise ValueError(f"pulsar {p}: basis width {Ts[p].shape[1]} is not supported with a block-diagonal N")
                 prep.append(blockn.prepare(toas[p], residuals[p], Nvecs[p], Ts[p], ci))
+                epochs.append(blockn.epochs(Nvecs[p], Ts[p].shape[0]))
                 n.append(prep[-1]["toas"].shape[0])
                 m.append(Ts[p].shape[1])
         else:
@@ -318,6 +326,8 @@ class Pack:
             check(lib.fastfp_pack_create(*head, *map(_ptr_array, (toas, residuals, Nvecs, Ts, mats)), *tail))
         pack = cls(h, P, device, nmfp, n, m)
         pack.blockn = block
+        if block:
+            pack.epochs = epochs
         return pack
 
     # -- sweeps -------------------------------------------------------------------------
@@ -401,7 +411,8 @@ class Pack:
         pack keeps them until the next call. ``R`` is at most :func:`max_residual_rows` of the pack's widths; an
         empty list of rows (``R == 0``) releases them."""
         if self.blockn:  # its TOAs are re-laid out by epoch (blockn.prepare); the library refuses these packs too
-            raise FastFpError("residual batches need a diagonal-N pack; this one has a block-diagonal N")
+            raise FastFpError("set_residuals needs a diagonal-N pack; this one has a block-diagonal N and takes its "
+                              "realisations through set_residuals_blockn")
         if len(residuals) != self.P:
             raise ValueError(f"residuals must be a list of {self.P} arrays (one per pulsar)")
         res = [as_f64(r) for r in residuals]
@@ -411,6 +422,50 @@ class Pack:
                 raise ValueError(f"residuals[{p}] must have shape (R, {self.n[p]}) with the same R for every pulsar; "
                                  f"got {r.shape}")
         check(load().fastfp_pack_set_residuals(self._h, R, _ptr_array(res), C.c_void_p(stream)))
+        self.R = R
+
+    def set_residuals_blockn(self, residuals, stream: int = 0) -> None:
+        """:meth:`set_residuals` for a block-diagonal N pack: ``residuals[p]`` is ``(R, n_p)`` (host) in the caller's
+        original TOA order, ``n_p`` the pulsar's TOA count before the epoch layout. The rows are laid out for the chunk
+        size of the residual kernel (``blockn.layout``), the Sherman-Morrison ``N^-1 r_k`` is applied on the host
+        (``blockn.solve_rows``) and ``fastfp_pack_set_residuals_blockn`` builds the packets. ``R`` is at most
+        ``max_residual_rows(m, blockn=True)``; ``R == 0`` releases the set."""
+        from . import blockn
+
+        if not self.blockn:
+            raise FastFpError("set_residuals_blockn needs a block-diagonal N pack; this one takes set_residuals")
+        if len(residuals) != self.P:
+            raise ValueError(f"residuals must be a list of {self.P} arrays (one per pulsar)")
+        res = [as_f64(r) for r in residuals]
+        R = res[0].shape[0] if res[0].ndim == 2 else -1
+        for p, r in enumerate(res):
+            if r.shape != (R, self.epochs[p].n):
+                raise ValueError(f"residuals[{p}] must have shape (R, {self.epochs[p].n}) with the same R for every "
+                                 f"pulsar; got {r.shape}")
+        lib = load()
+        P = self.P
+        i32pp, u8pp = C.POINTER(C.c_int32) * P, C.POINTER(C.c_ubyte) * P
+        if R == 0 or R > max_residual_rows(self.m, blockn=True):  # nothing to lay out: the library releases or refuses
+            check(lib.fastfp_pack_set_residuals_blockn(self._h, R, _int64_array(self.n), (c_double_p * P)(),
+                                                       (c_double_p * P)(), i32pp(), (c_double_p * P)(), u8pp(),
+                                                       C.c_void_p(stream)))
+            self.R = 0
+            return
+        n, raw, rw, sidx, sval, dm = [], [], [], [], [], []
+        for p in range(P):
+            ci = lib.fastfp_sweep_chunk_toas(-(-self.m[p] // 8) * 8 + -(-R // 8) * 8, 1)
+            lay = blockn.layout(self.epochs[p], ci)
+            order = lay["order"]
+            n.append(order.shape[0])
+            raw.append(blockn.relay(order, res[p]))
+            rw.append(blockn.relay(order, blockn.solve_rows(self.epochs[p], res[p])))
+            sidx.append(lay["slot_idx"])
+            sval.append(lay["slot_val"])
+            dm.append(lay["done_mask"])
+        check(lib.fastfp_pack_set_residuals_blockn(
+            self._h, R, _int64_array(n), _ptr_array(raw), _ptr_array(rw),
+            i32pp(*[a.ctypes.data_as(C.POINTER(C.c_int32)) for a in sidx]), _ptr_array(sval),
+            u8pp(*[a.ctypes.data_as(C.POINTER(C.c_ubyte)) for a in dm]), C.c_void_p(stream)))
         self.R = R
 
     def fp_sweep_residuals(self, freqs, out=None, stream: int = 0):

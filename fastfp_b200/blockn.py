@@ -83,11 +83,23 @@ def is_block(Nvec) -> bool:
     return all(hasattr(Nvec, a) for a in ("_nvec", "_jvec", "_slices"))
 
 
-def prepare(toas, res, Nvec, T, CI: int):
-    """Lay one pulsar out for a block-N pack. ``Nvec`` is a :class:`BlockNvec`-like object or a
-    1-D array (no epochs). Returns a dict of the arrays ``fastfp_pack_create_blockn`` takes."""
-    toas, res, T = (np.asarray(a, dtype=np.float64) for a in (toas, res, T))
-    n, m = T.shape
+@dataclass
+class Epochs:
+    """One pulsar's block-diagonal N as the layout and the Sherman-Morrison need it: the white variances ``nvec``,
+    the epochs ``slices`` as ``(start, stop)`` and ``beta_e = jvec_e / (1 + jvec_e * sum_e 1/nvec)``. A diagonal N
+    has no epochs."""
+
+    nvec: np.ndarray
+    slices: List[tuple]
+    beta: np.ndarray
+
+    @property
+    def n(self) -> int:
+        return self.nvec.shape[0]
+
+
+def epochs(Nvec, n: int) -> Epochs:
+    """The :class:`Epochs` of a :class:`BlockNvec`-like object or a 1-D array (no epochs) for ``n`` TOAs."""
     if is_block(Nvec):
         nvec = np.asarray(Nvec._nvec, dtype=np.float64)
         slices = [(int(s.start), int(s.stop)) for s in Nvec._slices]
@@ -101,15 +113,37 @@ def prepare(toas, res, Nvec, T, CI: int):
         if not 0 <= a < b <= n or covered[a:b].any():
             raise ValueError("block N: slices must be non-empty, in range and disjoint")
         covered[a:b] = True
-    ninv = 1.0 / nvec
-    # Sherman-Morrison applied to T and r, expressed as (N^-1 x) * nvec so the kernels' x/N recovers it
-    Tw, rw = T.copy(), res.copy()
     beta = np.zeros(len(slices))
     if slices:
         idx, eid, offs = _epoch_index([slice(a, b) for a, b in slices])
-        beta = jvec / (1.0 + jvec * np.add.reduceat(ninv[idx], offs))
-        Tw[idx] -= (beta[:, None] * np.add.reduceat(T[idx] * ninv[idx, None], offs, axis=0))[eid]
-        rw[idx] -= (beta * np.add.reduceat(res[idx] * ninv[idx], offs))[eid]
+        beta = jvec / (1.0 + jvec * np.add.reduceat(1.0 / nvec[idx], offs))
+    return Epochs(nvec, slices, beta)
+
+
+def solve_rows(ep: Epochs, X) -> np.ndarray:
+    """Sherman-Morrison of the ``R`` rows of ``X`` (``(R, n)``) at once, expressed as ``(N^-1 x_k) * nvec`` so the
+    kernels' ``x/N`` recovers ``N^-1 x_k``: the ``res_w`` of :func:`prepare`, row by row and bit for bit."""
+    X = np.asarray(X, dtype=np.float64)
+    out = X.copy()
+    if ep.slices:
+        idx, eid, offs = _epoch_index([slice(a, b) for a, b in ep.slices])
+        ninv = 1.0 / ep.nvec
+        out[:, idx] -= (ep.beta * np.add.reduceat(X[:, idx] * ninv[idx], offs, axis=1))[:, eid]
+    return out
+
+
+def layout(ep: Epochs, CI: int) -> dict:
+    """The TOA order of a block-N pack whose kernel takes chunks of ``CI`` TOAs, and its epoch slots.
+
+    TOAs are laid out as the epochs, each padded to a multiple of 4, then the TOAs outside any epoch, 4 at a time, then
+    padding k-blocks up to a multiple of ``CI``. Only that padded tail depends on ``CI``: two layouts of one pulsar agree
+    position by position on every real TOA (the residual batches of a block-N pack rely on it). Returns ``order``
+    (original TOA index, -1 for padding), ``slot_idx`` (slot 0..7 of a TOA's epoch inside its chunk, -1 if none),
+    ``slot_val`` (``sqrt(beta_e) / nvec_i``) and ``done_mask`` (per chunk, the slots whose epoch ends there)."""
+    n, slices, beta, nvec = ep.n, ep.slices, ep.beta, ep.nvec
+    covered = np.zeros(n, dtype=bool)
+    for (a, b) in slices:
+        covered[a:b] = True
     # groups of TOAs: epochs (padded to multiples of 4) then the uncovered TOAs, 4 at a time
     KB = CI // 4
     order: List[int] = []          # original TOA index or -1 (padding), length 4 * number of k-blocks
@@ -154,18 +188,46 @@ def prepare(toas, res, Nvec, T, CI: int):
                 carry[e] = s
     order = np.asarray(order, dtype=np.int64)
     real = order >= 0
-    npad = order.shape[0]
-    out_t = np.zeros(npad); out_r = np.zeros(npad); out_rw = np.zeros(npad)
-    out_n = np.full(npad, np.inf); out_T = np.zeros((npad, m))
-    out_t[real], out_r[real], out_rw[real] = toas[order[real]], res[order[real]], rw[order[real]]
-    out_n[real] = nvec[order[real]]
-    out_T[real] = Tw[order[real]]
     slot_idx = np.repeat(slot_of_kb, 4).astype(np.int32)
     slot_idx[~real] = -1
-    slot_val = np.zeros(npad)
+    slot_val = np.zeros(order.shape[0])
     ep_of_toa = np.repeat(np.asarray(kb_epoch), 4)
     sel = real & (ep_of_toa >= 0)
     slot_val[sel] = np.sqrt(beta[ep_of_toa[sel]]) / nvec[order[sel]]
     slot_idx[~sel] = -1
-    return dict(toas=out_t, res=out_r, res_w=out_rw, Nvec=out_n, T=np.ascontiguousarray(out_T),
-                slot_idx=np.ascontiguousarray(slot_idx), slot_val=slot_val, done_mask=np.ascontiguousarray(done))
+    return dict(order=order, slot_idx=np.ascontiguousarray(slot_idx), slot_val=slot_val,
+                done_mask=np.ascontiguousarray(done))
+
+
+def relay(order, X) -> np.ndarray:
+    """The columns of ``X`` (``(..., n)``) in the TOA order ``order`` of :func:`layout`, zero at padding."""
+    X = np.asarray(X, dtype=np.float64)
+    real = order >= 0
+    out = np.zeros(X.shape[:-1] + order.shape)
+    out[..., real] = X[..., order[real]]
+    return out
+
+
+def prepare(toas, res, Nvec, T, CI: int):
+    """Lay one pulsar out for a block-N pack. ``Nvec`` is a :class:`BlockNvec`-like object or a
+    1-D array (no epochs). Returns a dict of the arrays ``fastfp_pack_create_blockn`` takes."""
+    toas, res, T = (np.asarray(a, dtype=np.float64) for a in (toas, res, T))
+    n, m = T.shape
+    ep = epochs(Nvec, n)
+    nvec, ninv = ep.nvec, 1.0 / ep.nvec
+    # Sherman-Morrison applied to T and r, expressed as (N^-1 x) * nvec so the kernels' x/N recovers it
+    Tw = T.copy()
+    if ep.slices:
+        idx, eid, offs = _epoch_index([slice(a, b) for a, b in ep.slices])
+        Tw[idx] -= (ep.beta[:, None] * np.add.reduceat(T[idx] * ninv[idx, None], offs, axis=0))[eid]
+    rw = solve_rows(ep, res[None])[0]
+    lay = layout(ep, CI)
+    order = lay["order"]
+    real = order >= 0
+    out_n = np.full(order.shape[0], np.inf)
+    out_n[real] = nvec[order[real]]
+    out_T = np.zeros((order.shape[0], m))
+    out_T[real] = Tw[order[real]]
+    return dict(toas=relay(order, toas), res=relay(order, res), res_w=relay(order, rw), Nvec=out_n,
+                T=np.ascontiguousarray(out_T), slot_idx=lay["slot_idx"], slot_val=lay["slot_val"],
+                done_mask=lay["done_mask"])

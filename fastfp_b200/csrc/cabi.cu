@@ -455,7 +455,8 @@ int fastfp_pack_set_residuals(fastfp_pack_t* pk, int64_t R, const double* const*
   }
   if (pk->nmfp) { set_error("fastfp_pack_set_residuals needs a plain-Fp pack (fastfp_pack_create)"); return FASTFP_ERR_INVALID; }
   if (pk->ecorr) {
-    set_error("fastfp_pack_set_residuals: block-diagonal N packs are not supported");
+    set_error("fastfp_pack_set_residuals: a block-diagonal N pack takes its realisations in its own TOA layout "
+              "(fastfp_pack_set_residuals_blockn)");
     return FASTFP_ERR_UNSUPPORTED;
   }
   int wide = 0;
@@ -484,6 +485,57 @@ int fastfp_pack_set_residuals(fastfp_pack_t* pk, int64_t R, const double* const*
                              cudaMemcpyHostToDevice, c.st));
   }
   return build_res_packets(pk, R, d_res.get(), c.st);
+}
+
+// Residual batches of a block-diagonal N pack: the realisations in the TOA layout of the residual kernel's chunk size
+int fastfp_pack_set_residuals_blockn(fastfp_pack_t* pk, int64_t R, const int64_t* n, const double* const* residuals,
+                                     const double* const* residuals_w, const int32_t* const* slot_idx,
+                                     const double* const* slot_val, const unsigned char* const* done_mask,
+                                     void* stream) {
+  if (!pk || R < 0 || (R > 0 && (!n || !residuals || !residuals_w || !slot_idx || !slot_val || !done_mask))) {
+    set_error("fastfp_pack_set_residuals_blockn: null argument or negative R");
+    return FASTFP_ERR_INVALID;
+  }
+  if (pk->nmfp) {
+    set_error("fastfp_pack_set_residuals_blockn needs a plain-Fp pack (fastfp_pack_create_blockn without m_fix)");
+    return FASTFP_ERR_INVALID;
+  }
+  if (!pk->ecorr) {
+    set_error("fastfp_pack_set_residuals_blockn needs a block-diagonal N pack; a diagonal-N pack takes "
+              "fastfp_pack_set_residuals");
+    return FASTFP_ERR_INVALID;
+  }
+  int wide = 0;
+  for (int p = 0; p < pk->P; ++p)
+    if (pk->meta[p].m > pk->meta[wide].m) wide = p;
+  const int64_t rmax = MAX_M - 8 - (pk->meta[wide].m + 7) / 8 * 8;
+  if (R > rmax) {
+    set_error("fastfp_pack_set_residuals_blockn: R = " + std::to_string(R) + " exceeds the limit of " +
+              std::to_string(rmax) + " for this pack: its widest pulsar " + std::to_string(wide) + " (m = " +
+              std::to_string(pk->meta[wide].m) + ") and the 8 epoch-slot rows leave " + std::to_string(rmax) +
+              " of the sweep kernel's " + std::to_string(MAX_M) + " G rows");
+    return FASTFP_ERR_UNSUPPORTED;
+  }
+  for (int p = 0; p < pk->P && R > 0; ++p) {
+    if (!residuals[p] || !residuals_w[p] || !slot_idx[p] || !slot_val[p] || !done_mask[p]) {
+      set_error("fastfp_pack_set_residuals_blockn: null per-pulsar array");
+      return FASTFP_ERR_INVALID;
+    }
+    const int64_t m = pk->meta[p].m, ci = fastfp_sweep_chunk_toas((m + 7) / 8 * 8 + (R + 7) / 8 * 8, 1);
+    if (n[p] < 1 || n[p] > 0x7fffff00LL || n[p] % ci != 0) {
+      set_error("fastfp_pack_set_residuals_blockn: pulsar " + std::to_string(p) + ": the TOA count " +
+                std::to_string(n[p]) + " of the residual layout must be a positive multiple of its chunk size " +
+                std::to_string(ci) + " (fastfp_sweep_chunk_toas(roundup8(m) + roundup8(R), 1))");
+      return FASTFP_ERR_INVALID;
+    }
+  }
+  PackCall c(pk, stream);
+  if (int rc = c.select()) return rc;
+  FFP_CUDA(cudaStreamSynchronize(c.st));  // sweeps queued on this stream may still read the previous set
+  pk->res = {};
+  if (R == 0) return FASTFP_OK;
+  const ResBlockNHost bn{n, residuals, residuals_w, slot_idx, slot_val, done_mask};
+  return build_res_packets(pk, R, nullptr, c.st, &bn);
 }
 
 int fastfp_fp_sweep_residuals(const fastfp_pack_t* pk, const double* freqs, int64_t F, double* out, int flags,

@@ -251,10 +251,13 @@ struct PowerlawStaging {
 };
 
 // residual batch (fastfp_pack_set_residuals, DESIGN.md section 5d): per pulsar, the G rows followed by the R
-// realisations' w_k rows from row roundup8(m) on, in packets of the kernel configuration for that many rows
+// realisations' w_k rows from row roundup8(m) on, in packets of the kernel configuration for that many rows (block-N
+// packs, fastfp_pack_set_residuals_blockn: 8 more rows, the epoch slots, last; their TOAs in the layout of that
+// configuration's chunk size, with its own slot masks)
 struct ResidualBatch {
   DeviceBuf<double> packets;
   DeviceBuf<PulsarMeta> meta;
+  DeviceBuf<unsigned char> done_mask;  // block-N: per-chunk epoch-slot masks of the residual layout
   std::vector<Group> groups;
   mutable Scratch<double> terms;  // [R][P][F_batch] terms of one frequency batch
   int64_t R = 0;
@@ -312,9 +315,20 @@ int launch_fp_precompute(fastfp_pack* pk, const double* d_toas, const double* d_
                          const double* d_Nvec, const double* d_T, cudaStream_t st,
                          double* d_ur_keep = nullptr,  // [P][MAX_M], receives G r
                          const BlockNDev* bn = nullptr);
-// the residual packets of R realisations (d_res: per pulsar (R, n_p) row-major at R * raw_off) into pk->res, which the
-// caller has released
-int build_res_packets(fastfp_pack* pk, int64_t R, const double* d_res, cudaStream_t st);
+// host arrays of fastfp_pack_set_residuals_blockn: per pulsar, the residual layout's TOA count n[p], the (R, n[p])
+// realisations raw and as (N^-1 r_k) * Nvec, and that layout's slot indices and values (per TOA) and masks (per chunk)
+struct ResBlockNHost {
+  const int64_t* n;
+  const double* const* res;
+  const double* const* res_w;
+  const int32_t* const* slot_idx;
+  const double* const* slot_val;
+  const unsigned char* const* done_mask;
+};
+// the residual packets of R realisations into pk->res, which the caller has released. Diagonal N: d_res holds per
+// pulsar (R, n_p) row-major at R * raw_off. Block-N (bn set, d_res null): the arrays of bn, staged here.
+int build_res_packets(fastfp_pack* pk, int64_t R, const double* d_res, cudaStream_t st,
+                      const ResBlockNHost* bn = nullptr);
 // the pulsars of each kernel configuration as Groups with their indices on the device, appended to *out
 int upload_groups(const std::map<KernelCfg, std::vector<int>>& groups, std::vector<Group>* out);
 // fe.cu

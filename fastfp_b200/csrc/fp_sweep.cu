@@ -90,6 +90,7 @@ int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, con
 int launch_fp_sweep_res(const fastfp_pack* pk, const double* d_freqs, int64_t F, const ResOut& out, cudaStream_t st) {
   SweepArgs a = sweep_args(pk->res.packets.get(), pk->res.meta.get(), pk, d_freqs, F);
   a.res = out;
+  a.done_mask = pk->res.done_mask.get();  // block-N packs: the slot masks of the residual layout's chunks
   for (const Group& g : pk->res.groups)
     if (int rc = dispatch_group(pk, g.all(), a, SweepMode::Res, st)) return rc;
   return 0;

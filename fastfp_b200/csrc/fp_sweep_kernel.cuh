@@ -251,7 +251,9 @@ __device__ __forceinline__ void producer_loop(const SweepArgs& ar, SweepSmem<C>&
 }
 
 // Residual batches (DESIGN.md section 5d): rows from roundup8(m) on hold w_k = C^-1 r_k, so Y there is ((s|r_k),
-// (c|r_k)); one 2x2 system per (realisation, frequency) with the M of the frequency, which redB[fl][3] holds.
+// (c|r_k)); one 2x2 system per (realisation, frequency) with the M of the frequency, which redB[fl][3] holds. With a
+// block-diagonal N, w_k already carries the whole N^-1, so these rows need no epoch fold; the slot rows sit at mpad - 8,
+// after every realisation row read here.
 // acc[r][q]: as in consumer_loop's epilogue.
 template <class C>
 __device__ __forceinline__ void res_tail(const ResOut& out, int64_t F, const SweepSmem<C>& sm,
@@ -532,7 +534,6 @@ __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>&
 
 template <class C, SweepMode MODE, bool ECORR>
 __global__ void __launch_bounds__(C::NTHREADS, CTAS_PER_SM) fp_sweep_kernel(const SweepArgs ar) {
-  static_assert(!(MODE == SweepMode::Res && ECORR), "residual batches are diagonal-N only");
   extern __shared__ __align__(128) unsigned char smem_raw[];
   SweepSmem<C> sm(smem_raw);
   __shared__ int s_work;
@@ -585,14 +586,16 @@ int dispatch_sweep_w4(const fastfp_pack*, const GroupView&, const SweepArgs&, Sw
 int dispatch_sweep_wide(const fastfp_pack*, const GroupView&, const SweepArgs&, SweepMode, cudaStream_t);
 int dispatch_sweep_xwide(const fastfp_pack*, const GroupView&, const SweepArgs&, SweepMode, cudaStream_t);
 
-// five kernels per configuration: Fp and Nmfp, each with diagonal or block-diagonal N (pk->ecorr), and Res (diagonal N,
-// plain-Fp packs only)
+// six kernels per configuration: Fp, Nmfp and Res, each with diagonal or block-diagonal N (pk->ecorr; Res: plain-Fp packs
+// only, whose residual packets keep the 8 slot rows last, behind the realisations)
 #define FFP_SWEEP_CASE(NMBWv, NNBv, WMWv, CIv) FFP_SWEEP_CASE_W(NMBWv, NNBv, WMWv, CIv, 8, 16)
 #define FFP_SWEEP_CASE_W(NMBWv, NNBv, WMWv, CIv, NWCv, NWPv)                                       \
   if (g.cfg.nmbw == NMBWv && g.cfg.nnb == NNBv && g.cfg.wmw == WMWv && g.cfg.ci == CIv &&          \
       g.cfg.nwc == NWCv) {                                                                         \
     using Cfg_ = SweepCfg<NMBWv, NNBv, WMWv, CIv, NWCv, NWPv>;                                      \
-    if (mode == SweepMode::Res) return launch_sweep_cfg<Cfg_, SweepMode::Res, false>(pk, g, a, st);  \
+    if (mode == SweepMode::Res)                                                                    \
+      return pk->ecorr ? launch_sweep_cfg<Cfg_, SweepMode::Res, true>(pk, g, a, st)                \
+                       : launch_sweep_cfg<Cfg_, SweepMode::Res, false>(pk, g, a, st);              \
     if (mode == SweepMode::Nmfp)                                                                   \
       return pk->ecorr ? launch_sweep_cfg<Cfg_, SweepMode::Nmfp, true>(pk, g, a, st)               \
                        : launch_sweep_cfg<Cfg_, SweepMode::Nmfp, false>(pk, g, a, st);             \

@@ -174,7 +174,9 @@ def _tile_cost(rows: int) -> float:
     rows, times a per-row factor. On an H100 a tile row costs about the same in every configuration measured (0.49-0.51
     ms per row at C2 shapes for 40 to 384 rows) except the 8-frequency family with 10 row blocks per warp (640 rows),
     which costs 1.3-1.5 times as much per row (DESIGN.md section 5d). That family was measured at 6 row blocks (384
-    rows, no extra cost) and at 10; the 7 to 9 blocks in between were not measured and are given the 10-block factor."""
+    rows, no extra cost) and at 10; the 7 to 9 blocks in between were not measured and are given the 10-block factor.
+    These costs were measured with a diagonal N; block-N passes (8 more rows, the epoch slots, folded per epoch) are
+    modelled with the same factors, which is not measured."""
     for top, per_block in ((40, 8), (80, 8), (160, 16), (320, 32), (640, 64)):
         if rows <= top:
             nmbw = -(-rows // per_block)
@@ -182,13 +184,13 @@ def _tile_cost(rows: int) -> float:
     raise ValueError(f"{rows} rows exceed the sweep kernel")
 
 
-def batch_pass_rows(R: int, m) -> int:
+def batch_pass_rows(R: int, m, blockn: bool = False) -> int:
     """Realisations per pass of :meth:`FastFp.calculate_Fp_batch` for ``R`` realisations of pulsars of basis widths
     ``m``: of the even splits of ``R`` into passes the library takes (at most ``_cabi.max_residual_rows`` rows each),
-    the one with the least modelled cost, passes x :func:`_tile_cost` of ``roundup8(max m) + roundup8(rows)`` rows;
-    among equal costs the fewest passes."""
-    mr = -(-max(m) // 8) * 8
-    rmax = _cabi.max_residual_rows(m)
+    the one with the least modelled cost, passes x :func:`_tile_cost` of ``roundup8(max m) + roundup8(rows)`` rows
+    (``+ 8``, the epoch slots, for a block-diagonal N pack: ``blockn=True``); among equal costs the fewest passes."""
+    mr = -(-max(m) // 8) * 8 + (8 if blockn else 0)
+    rmax = _cabi.max_residual_rows(m, blockn)
     best = None
     for cap in sorted({min(R, rmax)} | set(range(8, min(R, rmax), 8))):
         npass = -(-R // cap)
@@ -261,9 +263,13 @@ class FastFp(_PackCache):
         uploaded pass by pass on every call, and each upload synchronises the stream, so with a CUDA-tensor ``fgw``
         such a call returns only when its last pass has been launched and is not asynchronous; the content hash of
         ``residuals`` is also taken on the calling thread before the first launch. The library takes at most ``_cabi.max_residual_rows`` rows per pass (568
-        at m = 72); ``R`` is split into passes of :func:`batch_pass_rows` rows, the split with the least modelled
+        at m = 72, 560 with a block-diagonal N); ``R`` is split into passes of :func:`batch_pass_rows` rows, the split with the least modelled
         sweep cost (measured per-row costs of the kernel configurations). The pass size selects the kernel configuration, so values can differ in the last bits
-        between different ``R``; within one ``R`` every row is computed alike wherever it sits."""
+        between different ``R``; within one ``R`` every row is computed alike wherever it sits.
+
+        A block-diagonal N (a ``BlockNvec`` or enterprise ``ShermanMorrison`` among the ``Nvecs``) works the same way:
+        the realisations, in the pulsars' original TOA order, are laid out by epoch and given the Sherman-Morrison
+        ``N^-1`` on the host (``_cabi.Pack.set_residuals_blockn``)."""
         R, passes = self._residual_passes(residuals)
         f, empty, stream, on_device = self._front_end(fgw)
         out = empty((R, f.shape[0]))
@@ -292,13 +298,15 @@ class FastFp(_PackCache):
         res_key = _fingerprint([res])
 
         def passes(pack, stream=0):
-            rows = batch_pass_rows(R, pack.m)
+            blockn = getattr(pack, "blockn", False)  # a pack without the attribute has a diagonal N
+            rows = batch_pass_rows(R, pack.m, blockn)
+            upload = pack.set_residuals_blockn if blockn else pack.set_residuals
             for lo in range(0, R, rows):
                 hi = min(R, lo + rows)
                 key = (res_key, lo, hi)
                 if self._res_pack is not pack or self._res_key != key:
                     self._res_pack, self._res_key = None, None
-                    pack.set_residuals([r[lo:hi] for r in res], stream=stream)
+                    upload([r[lo:hi] for r in res], stream=stream)
                     self._res_pack, self._res_key = pack, key
                 yield lo, hi
 

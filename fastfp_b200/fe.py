@@ -87,7 +87,8 @@ class FastFe(FastFp):
         stream for a float64 CUDA tensor. Row ``k`` is the sky maximum of Fe with residuals ``residuals[p][k]``, under
         the same rule (NaN loses, ties go to the lowest index, ``(nan, -1)`` where no position is finite). Values meet
         the parity bar of :meth:`calculate_Fe_skymax` but are not bit-identical to it (``fastfp_fe_skymax_residuals``,
-        DESIGN.md section 5e). One sky position is a targeted search at a known position."""
+        DESIGN.md section 5e). One sky position is a targeted search at a known position. A block-diagonal N among
+        the ``Nvecs`` works as in :meth:`calculate_Fp_batch`."""
         fplus, fcross = self._sky_grid(gwtheta, gwphi)
         R, passes = self._residual_passes(residuals)
         f, empty, stream, on_device = self._front_end(fgw)

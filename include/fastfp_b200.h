@@ -130,7 +130,7 @@ int fastfp_fe_skymax(const fastfp_pack_t* pack, const double* freqs, int64_t F, 
  *   packets until the next call or fastfp_pack_destroy; R == 0 releases them. fastfp_pack_bytes counts them. Each
  *   pulsar then needs roundup8(m_p) + roundup8(R) rows of the kernel's 640, so R <= 640 - roundup8(max_p m_p)
  *   (568 at m = 72). Returns FASTFP_ERR_INVALID for a NULL pack or array, R < 0 or an nmfp pack, and
- *   FASTFP_ERR_UNSUPPORTED for a block-N pack or an R above the limit (the message names the limit and the widest
+ *   FASTFP_ERR_UNSUPPORTED for a block-N pack (it takes fastfp_pack_set_residuals_blockn) or an R above the limit (the message names the limit and the widest
  *   pulsar). While it runs the call also holds a device staging copy of the realisations, R * sum_p n_p doubles
  *   (3.1 GB at R = 568 for 68 pulsars of 10^4 TOAs), on top of the packets it keeps (sum_p ceil(n_p / CI) * CI *
  *   (4 + MP) doubles, 3.5 GB in that case); the staging copy is freed before it returns.
@@ -143,6 +143,28 @@ int fastfp_fe_skymax(const fastfp_pack_t* pack, const double* freqs, int64_t F, 
  *   min(F, 2^27 / (R * P))) (at most 1 GiB unless R * P > 131 072), kept until the realisations are replaced or
  *   released, plus R * F doubles for host outputs in the pack's output buffer, kept until fastfp_pack_destroy. */
 int fastfp_pack_set_residuals(fastfp_pack_t* pack, int64_t R, const double* const* residuals, void* stream);
+/* fastfp_pack_set_residuals_blockn: the realisations of a block-diagonal N pack (fastfp_pack_create_blockn without
+ *   m_fix), for fastfp_fp_sweep_residuals and fastfp_fe_skymax_residuals. Each pulsar's residual packets hold the
+ *   basis rows, w_1 .. w_R from row roundup8(m_p) on and the 8 epoch-slot rows last: roundup8(m_p) + roundup8(R) + 8
+ *   rows, so R <= 632 - roundup8(max_p m_p) (560 at m = 72). That many rows usually select another kernel family than
+ *   the pack's, with another chunk size, so the realisations come in the TOA layout of that chunk size (the layout of
+ *   fastfp_pack_create_blockn, built for fastfp_sweep_chunk_toas(roundup8(m_p) + roundup8(R), 1) TOAs per chunk; it
+ *   agrees with the pack's layout position by position on every real TOA, and the pack's G rows and 1/N are paired
+ *   with it by position):
+ *     n[p]            TOA count of that layout, a multiple of its chunk size
+ *     residuals[p]    (R, n[p]) row-major, the raw realisations (0 on padding TOAs)
+ *     residuals_w[p]  (R, n[p]) row-major, (N^-1 r_k) * Nvec as residuals_w of fastfp_pack_create_blockn
+ *     slot_idx[p], slot_val[p]  per TOA of that layout, done_mask[p] per chunk, as for fastfp_pack_create_blockn
+ *   R == 0 releases the set. fastfp_pack_bytes counts the packets and the slot masks. Returns FASTFP_ERR_INVALID for a
+ *   NULL argument, R < 0, an nmfp pack, a diagonal-N pack (it takes fastfp_pack_set_residuals) or an n[p] that is not a
+ *   positive multiple of the chunk size, and FASTFP_ERR_UNSUPPORTED for an R above the limit (the message names the
+ *   limit and the widest pulsar). While it runs the call holds device staging copies of both arrays, 2 R * sum_p n_p
+ *   doubles, twice the staging of fastfp_pack_set_residuals (5.6 GB at R = 560 for 68 pulsars of 10^4 TOAs), plus the
+ *   slot arrays, 12 bytes per TOA; they are freed before it returns. */
+int fastfp_pack_set_residuals_blockn(fastfp_pack_t* pack, int64_t R, const int64_t* n, const double* const* residuals,
+                                     const double* const* residuals_w, const int32_t* const* slot_idx,
+                                     const double* const* slot_val, const unsigned char* const* done_mask,
+                                     void* stream);
 int fastfp_fp_sweep_residuals(const fastfp_pack_t* pack, const double* freqs, int64_t F, double* out, int flags,
                               void* stream);
 
@@ -155,7 +177,7 @@ int fastfp_fp_sweep_residuals(const fastfp_pack_t* pack, const double* freqs, in
  *   the pulsars, and the 4x4 solve multiplies by reciprocal pivots (DESIGN.md section 5e). It always runs the fp64
  *   kernel, whatever fastfp_pack_path says. fplus, fcross: host arrays (S, P) row-major. flags as for fastfp_fp_sweep;
  *   FASTFP_OUT_ON_DEVICE covers both outputs. Returns FASTFP_ERR_INVALID for a NULL argument, a negative size, an nmfp
- *   pack, a pack with no realisations set (block-N packs cannot hold them), or S == 0 with F > 0; F == 0 returns
+ *   pack, a pack with no realisations set, or S == 0 with F > 0; F == 0 returns
  *   FASTFP_OK and writes nothing.
  *   Device scratch, grown on demand and kept until fastfp_pack_destroy: the realisations' inner products of one
  *   frequency batch, 2 R P F_batch doubles in the residual terms buffer (kept until the realisations are replaced or
@@ -227,7 +249,8 @@ int fastfp_powerlaw_phiinv(const fastfp_pack_t* pack, const double* const* Ffreq
  *   residuals_w[p] = (N^-1 r) * Nvec,  Ts[p] = (N^-1 T) * Nvec row-wise,  Nvecs[p] = diagonal part
  *   (inf on padding TOAs);  mats[p] = sigma_p (m_fix == NULL: plain Fp) or TNT_p (nmfp, with m_fix /
  *   phiinv_fix as in fastfp_nmfp_pack_create), both formed with the block N.
- * The resulting pack is used with fastfp_fp_sweep / fastfp_nmfp_sweep unchanged.
+ * The resulting pack is used with fastfp_fp_sweep / fastfp_nmfp_sweep unchanged; a plain-Fp one takes residual
+ * batches through fastfp_pack_set_residuals_blockn.
  * The epoch slots take 8 rows of the G tile after the basis rows (roundup8(m) + 8 in all), so a block-N pulsar
  * has m <= 632: fastfp_sweep_chunk_toas(m, 1) returns 0 above that and fastfp_pack_create_blockn returns
  * FASTFP_ERR_UNSUPPORTED. */
