@@ -108,11 +108,29 @@ SYMBOLS = {
 MAX_M = 640  # G rows of the widest sweep kernel (csrc/ffp_internal.cuh)
 
 
+def sweep_rows(m: int, R: int = 0, blockn: bool = False) -> int:
+    """G rows of the sweep kernel a pulsar of basis width ``m`` takes: its basis rows, then ``R`` residual realisations
+    from row ``roundup8(m)`` on, then with a block-diagonal N the 8 epoch-slot rows (csrc/ffp_internal.cuh)."""
+    return -(-m // 8) * 8 + -(-R // 8) * 8 + (8 if blockn else 0)
+
+
 def max_residual_rows(m, blockn: bool = False) -> int:
     """Most residual realisations ``fastfp_pack_set_residuals`` takes for pulsars of basis widths ``m``: every pulsar
-    needs ``roundup8(m_p) + roundup8(R)`` of the sweep kernel's ``MAX_M`` G rows. A block-diagonal N pack
+    needs :func:`sweep_rows` of the sweep kernel's ``MAX_M`` G rows. A block-diagonal N pack
     (``fastfp_pack_set_residuals_blockn``) needs 8 more, the epoch slots."""
-    return MAX_M - -(-max(m) // 8) * 8 - (8 if blockn else 0)
+    return MAX_M - sweep_rows(max(m), 0, blockn)
+
+
+def check_realisations(residuals, n):
+    """``residuals``, a list of one ``(R, n[p])`` array per pulsar with the same ``R``, as float64 arrays, and ``R``."""
+    if len(residuals) != len(n):
+        raise ValueError(f"residuals must be a list of {len(n)} arrays (one per pulsar)")
+    res = [as_f64(r) for r in residuals]
+    R = res[0].shape[0] if res[0].ndim == 2 else -1
+    for p, r in enumerate(res):
+        if r.shape != (R, n[p]):
+            raise ValueError(f"residuals[{p}] must have shape (R, {n[p]}) with the same R for every pulsar; got {r.shape}")
+    return res, R
 
 
 class FastFpError(RuntimeError):
@@ -413,14 +431,7 @@ class Pack:
         if self.blockn:  # its TOAs are re-laid out by epoch (blockn.prepare); the library refuses these packs too
             raise FastFpError("set_residuals needs a diagonal-N pack; this one has a block-diagonal N and takes its "
                               "realisations through set_residuals_blockn")
-        if len(residuals) != self.P:
-            raise ValueError(f"residuals must be a list of {self.P} arrays (one per pulsar)")
-        res = [as_f64(r) for r in residuals]
-        R = res[0].shape[0] if res[0].ndim == 2 else -1
-        for p, r in enumerate(res):
-            if r.shape != (R, self.n[p]):
-                raise ValueError(f"residuals[{p}] must have shape (R, {self.n[p]}) with the same R for every pulsar; "
-                                 f"got {r.shape}")
+        res, R = check_realisations(residuals, self.n)
         check(load().fastfp_pack_set_residuals(self._h, R, _ptr_array(res), C.c_void_p(stream)))
         self.R = R
 
@@ -434,14 +445,7 @@ class Pack:
 
         if not self.blockn:
             raise FastFpError("set_residuals_blockn needs a block-diagonal N pack; this one takes set_residuals")
-        if len(residuals) != self.P:
-            raise ValueError(f"residuals must be a list of {self.P} arrays (one per pulsar)")
-        res = [as_f64(r) for r in residuals]
-        R = res[0].shape[0] if res[0].ndim == 2 else -1
-        for p, r in enumerate(res):
-            if r.shape != (R, self.epochs[p].n):
-                raise ValueError(f"residuals[{p}] must have shape (R, {self.epochs[p].n}) with the same R for every "
-                                 f"pulsar; got {r.shape}")
+        res, R = check_realisations(residuals, [ep.n for ep in self.epochs])
         lib = load()
         P = self.P
         i32pp, u8pp = C.POINTER(C.c_int32) * P, C.POINTER(C.c_ubyte) * P
@@ -453,7 +457,7 @@ class Pack:
             return
         n, raw, rw, sidx, sval, dm = [], [], [], [], [], []
         for p in range(P):
-            ci = lib.fastfp_sweep_chunk_toas(-(-self.m[p] // 8) * 8 + -(-R // 8) * 8, 1)
+            ci = lib.fastfp_sweep_chunk_toas(sweep_rows(self.m[p], R), 1)
             lay = blockn.layout(self.epochs[p], ci)
             order = lay["order"]
             n.append(order.shape[0])

@@ -2,7 +2,6 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
-#include <map>
 
 #include "../../include/fastfp_b200.h"
 #include "ffp_internal.cuh"
@@ -50,32 +49,25 @@ static int pack_layout(fastfp_pack* pk, int P, const int64_t* n, const int64_t* 
                        const int64_t* m_fix, const double* const* toas, bool blockn = false) {
   pk->P = P;
   pk->meta.resize(P);
-  int64_t pk_off = 0, L_off = 0, raw_off = 0, T_off = 0, dm_off = 0;
+  int64_t L_off = 0, raw_off = 0, T_off = 0, dm_off = 0;
   int var_off = 0;
   pk->ecorr = blockn;
-  std::map<KernelCfg, std::vector<int>> groups;
+  PacketLayout lay;
   for (int p = 0; p < P; ++p) {
     if (n[p] < 1 || m[p] < 1 || n[p] > 0x7fffff00LL) {
       set_error("pulsar " + std::to_string(p) + ": n and m must be positive");
       return FASTFP_ERR_INVALID;
     }
-    KernelCfg kc{};
-    // block-diagonal N: one more block of 8 rows (the epoch slots) after the basis rows
-    const int m_rows = blockn ? ((int)m[p] + 7) / 8 * 8 + 8 : (int)m[p];
-    if (m[p] > MAX_M || !sweep_config(m_rows, &kc)) {
+    PulsarMeta& pm = pk->meta[p];
+    pm.n = (int)n[p];
+    if (m[p] > MAX_M || !lay.place(p, sweep_rows((int)m[p], 0, blockn), &pm)) {
       set_error("pulsar " + std::to_string(p) + ": basis width m=" + std::to_string(m[p]) +
                 (blockn ? " exceeds the block-N maximum " + std::to_string(MAX_M - 8) + " (the widest kernel has " +
                               std::to_string(MAX_M) + " rows, 8 of them hold the epoch slots)"
                         : " exceeds the supported maximum " + std::to_string(MAX_M)));
       return FASTFP_ERR_UNSUPPORTED;
     }
-    PulsarMeta& pm = pk->meta[p];
-    pm.n = (int)n[p];
     pm.m = (int)m[p];
-    pm.ci = kc.ci;
-    pm.nch = (int)((n[p] + kc.ci - 1) / kc.ci);
-    pm.mpad = kc.mp();
-    pm.pk_off = pk_off;
     pm.L_off = L_off;
     pm.raw_off = raw_off;
     pm.T_off = T_off;
@@ -87,11 +79,11 @@ static int pack_layout(fastfp_pack* pk, int P, const int64_t* n, const int64_t* 
     }
     pm.var_off = var_off;
     pm.dm_off = dm_off;
-    if (blockn && n[p] % kc.ci != 0) {
+    if (blockn && pm.n % pm.ci != 0) {
       set_error("block-N pack: the TOA count must be a multiple of the chunk size (fastfp_sweep_chunk_toas)");
       return FASTFP_ERR_INVALID;
     }
-    dm_off += (n[p] + kc.ci - 1) / kc.ci;
+    dm_off += pm.nch;
     pm.tabs_max = 0.0;
     if (!toas[p]) { set_error("null toas"); return FASTFP_ERR_INVALID; }
     for (int64_t i = 0; i < n[p]; ++i) {
@@ -101,17 +93,15 @@ static int pack_layout(fastfp_pack* pk, int P, const int64_t* n, const int64_t* 
     }
     var_off += pm.mvar;
     pk->mvar_max = std::max(pk->mvar_max, pm.mvar);
-    pk_off += (int64_t)pm.nch * pm.ci * (4 + pm.mpad);
     L_off += (int64_t)pm.m * pm.m;
     raw_off += pm.n;
     T_off += (int64_t)pm.n * pm.m;
-    groups[kc].push_back(p);
   }
   pk->mvar_total = var_off;
   PackCore& c = pk->core;
   FFP_CUDA(dev_alloc(&c.meta, (size_t)P));
   FFP_CUDA(cudaMemcpy(c.meta.get(), pk->meta.data(), sizeof(PulsarMeta) * P, cudaMemcpyHostToDevice));
-  FFP_CUDA(dev_alloc(&c.packets, (size_t)pk_off));
+  FFP_CUDA(dev_alloc(&c.packets, (size_t)lay.size));
   FFP_CUDA(dev_alloc(&c.L, (size_t)L_off));
   FFP_CUDA(dev_alloc(&c.info, (size_t)P));
   FFP_CUDA(cudaMemset(c.info.get(), 0, sizeof(int) * P));
@@ -119,8 +109,8 @@ static int pack_layout(fastfp_pack* pk, int P, const int64_t* n, const int64_t* 
   const size_t slab_doubles = (size_t)CTAS_PER_SM * pk->num_sms * sweep_max_slab_doubles();
   FFP_CUDA(dev_alloc(&c.slab, slab_doubles));
   FFP_CUDA(dev_alloc(&c.counter, 1));
-  pk->bytes = pk_off * 8 + L_off * 8 + (int64_t)sizeof(PulsarMeta) * P + (int64_t)slab_doubles * 8;
-  return upload_groups(groups, &pk->groups);
+  pk->bytes = lay.size * 8 + L_off * 8 + (int64_t)sizeof(PulsarMeta) * P + (int64_t)slab_doubles * 8;
+  return lay.upload(&pk->groups);
 }
 
 // which: 0 = length n_p, 1 = n_p*m_p (T), 2 = m_p*m_p
@@ -309,6 +299,32 @@ struct ScratchLayout {
   }
 };
 
+// The limit of a residual batch: every pulsar takes sweep_rows(m, R, blockn) of the kernel's MAX_M G rows, so the widest
+// one bounds R. FASTFP_ERR_UNSUPPORTED with a message that names the limit and that pulsar for an R above it.
+static int check_res_limit(const fastfp_pack* pk, int64_t R, const char* fn) {
+  int wide = 0;
+  for (int p = 0; p < pk->P; ++p)
+    if (pk->meta[p].m > pk->meta[wide].m) wide = p;
+  const int64_t rmax = MAX_M - sweep_rows(pk->meta[wide].m, 0, pk->ecorr);
+  if (R <= rmax) return FASTFP_OK;
+  set_error(std::string(fn) + ": R = " + std::to_string(R) + " exceeds the limit of " + std::to_string(rmax) +
+            " for this pack: its widest pulsar " + std::to_string(wide) + " (m = " + std::to_string(pk->meta[wide].m) +
+            (pk->ecorr ? ") and the 8 epoch-slot rows leave " : ") leaves ") + std::to_string(rmax) +
+            " of the sweep kernel's " + std::to_string(MAX_M) + " G rows");
+  return FASTFP_ERR_UNSUPPORTED;
+}
+
+// Replaces the pack's residual batch with the R realisations of h (R == 0: none), once the sweeps queued on the stream,
+// which may still read the previous set, are done
+static int replace_res(fastfp_pack* pk, int64_t R, const ResHost& h, void* stream) {
+  PackCall c(pk, stream);
+  if (int rc = c.select()) return rc;
+  FFP_CUDA(cudaStreamSynchronize(c.st));
+  pk->res = {};
+  if (R == 0) return FASTFP_OK;
+  return build_res_packets(pk, R, h, c.st);
+}
+
 }  // namespace ffp
 
 using namespace ffp;
@@ -374,8 +390,7 @@ int fastfp_nmfp_pack_create(int device, int P, const int64_t* n, const int64_t* 
 
 int fastfp_sweep_chunk_toas(int64_t m, int blockn) {
   KernelCfg kc{};
-  const int64_t m_rows = blockn ? (m + 7) / 8 * 8 + 8 : m;
-  if (m < 1 || m > MAX_M || !sweep_config((int)m_rows, &kc)) return 0;
+  if (m < 1 || m > MAX_M || !sweep_config(sweep_rows((int)m, 0, blockn != 0), &kc)) return 0;
   return kc.ci;
 }
 
@@ -432,7 +447,7 @@ static int fp_run(const fastfp_pack* pk, const double* freqs, int64_t F, double*
     for (int64_t lo = 0; lo < F; lo += FB) {
       const int64_t fb = std::min(FB, F - lo);
       if (int rc = launch_sweep(pk, d_freqs + lo, fb, FpOut{pk->terms.get(), nullptr}, c.st)) return rc;
-      if (int rc = launch_reduce_terms(pk->terms.get(), P, fb, d_out + lo, c.st)) return rc;
+      if (int rc = launch_reduce_terms_rows(pk->terms.get(), 1, P, fb, d_out + lo, F, c.st)) return rc;
     }
   }
   return c.finish(flags, nout, out, d_out, false);
@@ -459,32 +474,13 @@ int fastfp_pack_set_residuals(fastfp_pack_t* pk, int64_t R, const double* const*
               "(fastfp_pack_set_residuals_blockn)");
     return FASTFP_ERR_UNSUPPORTED;
   }
-  int wide = 0;
+  std::vector<int64_t> n(pk->P);
   for (int p = 0; p < pk->P; ++p) {
     if (R > 0 && !residuals[p]) { set_error("fastfp_pack_set_residuals: null per-pulsar array"); return FASTFP_ERR_INVALID; }
-    if (pk->meta[p].m > pk->meta[wide].m) wide = p;
+    n[p] = pk->meta[p].n;
   }
-  const int64_t rmax = MAX_M - (pk->meta[wide].m + 7) / 8 * 8;
-  if (R > rmax) {
-    set_error("fastfp_pack_set_residuals: R = " + std::to_string(R) + " exceeds the limit of " + std::to_string(rmax) +
-              " for this pack: its widest pulsar " + std::to_string(wide) + " (m = " + std::to_string(pk->meta[wide].m) +
-              ") leaves " + std::to_string(rmax) + " of the sweep kernel's " + std::to_string(MAX_M) + " G rows");
-    return FASTFP_ERR_UNSUPPORTED;
-  }
-  PackCall c(pk, stream);
-  if (int rc = c.select()) return rc;
-  FFP_CUDA(cudaStreamSynchronize(c.st));  // sweeps queued on this stream may still read the previous set
-  pk->res = {};
-  if (R == 0) return FASTFP_OK;
-  const int64_t n_tot = pk->meta.back().raw_off + pk->meta.back().n;
-  DeviceBuf<double> d_res;
-  FFP_CUDA(dev_alloc(&d_res, (size_t)(R * n_tot)));
-  for (int p = 0; p < pk->P; ++p) {
-    const PulsarMeta& pm = pk->meta[p];
-    FFP_CUDA(cudaMemcpyAsync(d_res.get() + R * pm.raw_off, residuals[p], (size_t)(R * pm.n) * 8,
-                             cudaMemcpyHostToDevice, c.st));
-  }
-  return build_res_packets(pk, R, d_res.get(), c.st);
+  if (int rc = check_res_limit(pk, R, "fastfp_pack_set_residuals")) return rc;
+  return replace_res(pk, R, {n.data(), residuals, residuals, nullptr, nullptr, nullptr}, stream);
 }
 
 // Residual batches of a block-diagonal N pack: the realisations in the TOA layout of the residual kernel's chunk size
@@ -505,37 +501,22 @@ int fastfp_pack_set_residuals_blockn(fastfp_pack_t* pk, int64_t R, const int64_t
               "fastfp_pack_set_residuals");
     return FASTFP_ERR_INVALID;
   }
-  int wide = 0;
-  for (int p = 0; p < pk->P; ++p)
-    if (pk->meta[p].m > pk->meta[wide].m) wide = p;
-  const int64_t rmax = MAX_M - 8 - (pk->meta[wide].m + 7) / 8 * 8;
-  if (R > rmax) {
-    set_error("fastfp_pack_set_residuals_blockn: R = " + std::to_string(R) + " exceeds the limit of " +
-              std::to_string(rmax) + " for this pack: its widest pulsar " + std::to_string(wide) + " (m = " +
-              std::to_string(pk->meta[wide].m) + ") and the 8 epoch-slot rows leave " + std::to_string(rmax) +
-              " of the sweep kernel's " + std::to_string(MAX_M) + " G rows");
-    return FASTFP_ERR_UNSUPPORTED;
-  }
+  if (int rc = check_res_limit(pk, R, "fastfp_pack_set_residuals_blockn")) return rc;
   for (int p = 0; p < pk->P && R > 0; ++p) {
     if (!residuals[p] || !residuals_w[p] || !slot_idx[p] || !slot_val[p] || !done_mask[p]) {
       set_error("fastfp_pack_set_residuals_blockn: null per-pulsar array");
       return FASTFP_ERR_INVALID;
     }
-    const int64_t m = pk->meta[p].m, ci = fastfp_sweep_chunk_toas((m + 7) / 8 * 8 + (R + 7) / 8 * 8, 1);
-    if (n[p] < 1 || n[p] > 0x7fffff00LL || n[p] % ci != 0) {
+    KernelCfg kc{};
+    if (!sweep_config(sweep_rows(pk->meta[p].m, R, true), &kc) || n[p] < 1 || n[p] > 0x7fffff00LL ||
+        n[p] % kc.ci != 0) {
       set_error("fastfp_pack_set_residuals_blockn: pulsar " + std::to_string(p) + ": the TOA count " +
                 std::to_string(n[p]) + " of the residual layout must be a positive multiple of its chunk size " +
-                std::to_string(ci) + " (fastfp_sweep_chunk_toas(roundup8(m) + roundup8(R), 1))");
+                std::to_string(kc.ci) + " (fastfp_sweep_chunk_toas(roundup8(m) + roundup8(R), 1))");
       return FASTFP_ERR_INVALID;
     }
   }
-  PackCall c(pk, stream);
-  if (int rc = c.select()) return rc;
-  FFP_CUDA(cudaStreamSynchronize(c.st));  // sweeps queued on this stream may still read the previous set
-  pk->res = {};
-  if (R == 0) return FASTFP_OK;
-  const ResBlockNHost bn{n, residuals, residuals_w, slot_idx, slot_val, done_mask};
-  return build_res_packets(pk, R, nullptr, c.st, &bn);
+  return replace_res(pk, R, {n, residuals, residuals_w, slot_idx, slot_val, done_mask}, stream);
 }
 
 int fastfp_fp_sweep_residuals(const fastfp_pack_t* pk, const double* freqs, int64_t F, double* out, int flags,

@@ -26,6 +26,12 @@ constexpr int VST = 16;        // TOA-vector ring depth (t | 1/N | w; TMA -> pro
 constexpr int FLUSH_TOAS = 512;  // level-1 accumulation block, in TOAs
 constexpr int MAX_M = 640;     // widest basis the sweep kernel handles (8 warp rows x 10 blocks of 8 rows)
 
+// G rows a pulsar of basis width m takes in the sweep kernel: its basis rows, then R residual realisations from row
+// roundup8(m) on (residual batches, DESIGN.md section 5d), then with a block-diagonal N the 8 epoch-slot rows last
+inline int sweep_rows(int m, int64_t R, bool blockn) {
+  return (m + 7) / 8 * 8 + (int)((R + 7) / 8 * 8) + (blockn ? 8 : 0);
+}
+
 // Sweep configuration. The contraction runs on the fp64 MMA path (mma.sync.m16n8k4.f64, basis rows on the N side): a
 // warp owns NMBW row blocks (8 basis rows each) x NNB/2 tiles of 8 frequencies x {sin, cos} (the 16 MMA rows), i.e.
 // 4*NNB frequencies; WMW consumer warps split the rows, NWC/WMW split the frequencies of the tile.
@@ -251,9 +257,9 @@ struct PowerlawStaging {
 };
 
 // residual batch (fastfp_pack_set_residuals, DESIGN.md section 5d): per pulsar, the G rows followed by the R
-// realisations' w_k rows from row roundup8(m) on, in packets of the kernel configuration for that many rows (block-N
-// packs, fastfp_pack_set_residuals_blockn: 8 more rows, the epoch slots, last; their TOAs in the layout of that
-// configuration's chunk size, with its own slot masks)
+// realisations' w_k rows, in packets of the kernel configuration for its sweep_rows (block-N packs,
+// fastfp_pack_set_residuals_blockn: with the epoch slots last; their TOAs in the layout of that configuration's chunk
+// size, with its own slot masks)
 struct ResidualBatch {
   DeviceBuf<double> packets;
   DeviceBuf<PulsarMeta> meta;
@@ -315,9 +321,10 @@ int launch_fp_precompute(fastfp_pack* pk, const double* d_toas, const double* d_
                          const double* d_Nvec, const double* d_T, cudaStream_t st,
                          double* d_ur_keep = nullptr,  // [P][MAX_M], receives G r
                          const BlockNDev* bn = nullptr);
-// host arrays of fastfp_pack_set_residuals_blockn: per pulsar, the residual layout's TOA count n[p], the (R, n[p])
-// realisations raw and as (N^-1 r_k) * Nvec, and that layout's slot indices and values (per TOA) and masks (per chunk)
-struct ResBlockNHost {
+// host arrays of a residual batch: per pulsar, the residual layout's TOA count n[p] and the (R, n[p]) realisations raw
+// and as (N^-1 r_k) * Nvec (diagonal N: the pack's n, and res_w == res); block-N packs also that layout's slot indices
+// and values (per TOA) and masks (per chunk), null otherwise
+struct ResHost {
   const int64_t* n;
   const double* const* res;
   const double* const* res_w;
@@ -325,12 +332,17 @@ struct ResBlockNHost {
   const double* const* slot_val;
   const unsigned char* const* done_mask;
 };
-// the residual packets of R realisations into pk->res, which the caller has released. Diagonal N: d_res holds per
-// pulsar (R, n_p) row-major at R * raw_off. Block-N (bn set, d_res null): the arrays of bn, staged here.
-int build_res_packets(fastfp_pack* pk, int64_t R, const double* d_res, cudaStream_t st,
-                      const ResBlockNHost* bn = nullptr);
-// the pulsars of each kernel configuration as Groups with their indices on the device, appended to *out
-int upload_groups(const std::map<KernelCfg, std::vector<int>>& groups, std::vector<Group>* out);
+// the residual packets of R realisations into pk->res, which the caller has released
+int build_res_packets(fastfp_pack* pk, int64_t R, const ResHost& h, cudaStream_t st);
+// packets of pulsars one after another, each in the kernel configuration for its number of G rows
+struct PacketLayout {
+  int64_t size = 0;                              // doubles
+  std::map<KernelCfg, std::vector<int>> groups;  // the pulsars of each configuration
+  // pulsar p with `rows` G rows and pm->n TOAs: sets pm's ci, nch, mpad and pk_off; false if no configuration has them
+  bool place(int p, int rows, PulsarMeta* pm);
+  // the groups with their indices on the device, appended to *out
+  int upload(std::vector<Group>* out) const;
+};
 // fe.cu
 int launch_fe_combine(const double* d_inner, int P, int64_t F, const double* d_fplus, const double* d_fcross, int64_t S,
                       double* d_out, int64_t out_ld, cudaStream_t st);
@@ -542,10 +554,9 @@ int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, con
                     bool rest_only = false);
 int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, const NmfpTiles& out, cudaStream_t st,
                     bool rest_only = false);
-int launch_reduce_terms(const double* d_terms, int P, int64_t F, double* d_out, cudaStream_t st);
-// residual batches: the sweep over the pack's residual packets and the pulsar sum of each row of its [R][P][F] terms
-// into out[k * ld + f] (fp_sweep.cu)
+// residual batches: the sweep over the pack's residual packets (fp_sweep.cu)
 int launch_fp_sweep_res(const fastfp_pack* pk, const double* d_freqs, int64_t F, const ResOut& out, cudaStream_t st);
+// the pulsar sum of each row of [R][P][F] terms into out[k * ld + f] (R = 1: the terms of a plain sweep)
 int launch_reduce_terms_rows(const double* d_terms, int R, int P, int64_t F, double* d_out, int64_t ld,
                              cudaStream_t st);
 // fp_sweep_i8.cu

@@ -25,16 +25,6 @@ bool sweep_config(int m, KernelCfg* c) {
 
 int sweep_max_slab_doubles() { return (40 + 12) * 12 * 32 + 10 * NTP; }  // NACC <= 80, XW <= 2, at most 12 consumer warps
 
-// out[f] = sum over pulsars in pulsar order, starting from 0 (fastfp.py:71,90).
-__global__ void reduce_terms_kernel(const double* __restrict__ terms, int P, int64_t F,
-                                    double* __restrict__ out) {
-  const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= F) return;
-  double acc = 0.0;
-  for (int p = 0; p < P; ++p) acc += terms[(size_t)p * F + f];
-  out[f] = acc;
-}
-
 static int dispatch_group(const fastfp_pack* pk, const GroupView& g, const SweepArgs& a, SweepMode mode,
                           cudaStream_t st) {
   if (g.cfg.wmw == 8) return dispatch_sweep_xwide(pk, g, a, mode, st);
@@ -96,7 +86,7 @@ int launch_fp_sweep_res(const fastfp_pack* pk, const double* d_freqs, int64_t F,
   return 0;
 }
 
-// out[k * ld + f] = sum over pulsars of terms[k][p][f], in pulsar order from 0 (as reduce_terms_kernel)
+// out[k * ld + f] = sum over pulsars of terms[k][p][f], in pulsar order from 0 (fastfp.py:71,90)
 __global__ void reduce_terms_rows_kernel(const double* __restrict__ terms, int P, int64_t F,
                                          double* __restrict__ out, int64_t ld) {
   const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -110,13 +100,6 @@ __global__ void reduce_terms_rows_kernel(const double* __restrict__ terms, int P
 int launch_reduce_terms_rows(const double* d_terms, int R, int P, int64_t F, double* d_out, int64_t ld,
                              cudaStream_t st) {
   reduce_terms_rows_kernel<<<dim3((unsigned)((F + 255) / 256), (unsigned)R), 256, 0, st>>>(d_terms, P, F, d_out, ld);
-  g_launches += 1;
-  FFP_CUDA(cudaGetLastError());
-  return 0;
-}
-
-int launch_reduce_terms(const double* d_terms, int P, int64_t F, double* d_out, cudaStream_t st) {
-  reduce_terms_kernel<<<(unsigned)((F + 255) / 256), 256, 0, st>>>(d_terms, P, F, d_out);
   g_launches += 1;
   FFP_CUDA(cudaGetLastError());
   return 0;

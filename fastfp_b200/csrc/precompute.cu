@@ -177,9 +177,9 @@ int launch_fp_precompute(fastfp_pack* pk, const double* d_toas, const double* d_
 // ---- residual batches (DESIGN.md section 5d) ---------------------------------------------------------
 // R realisations r_k of the residuals enter the sweep only through w_k = C^-1 r_k = r_k / N - G^T (G r_k). Their
 // packets hold, per pulsar, the G rows of the pack and then w_1 .. w_R as rows roundup8(m) .. roundup8(m) + R - 1,
-// laid out for the kernel configuration of roundup8(m) + roundup8(R) rows (its own CI and MP). A block-N pack adds the 8
-// epoch-slot rows last, at mpad - 8, where the ECORR sweep looks for them: roundup8(m) + roundup8(R) + 8 rows, in the
-// TOA layout of that configuration's chunk size (blockn.layout), which can differ from the pack's.
+// laid out for the kernel configuration of its sweep_rows (its own CI and MP). A block-N pack has the 8 epoch-slot rows
+// last, at mpad - 8, where the ECORR sweep looks for them, in the TOA layout of that configuration's chunk size
+// (blockn.layout), which can differ from the pack's.
 
 // G[j][i] of pulsar pm in the pack's packets
 __device__ __forceinline__ double g_at(const double* packets, const PulsarMeta& pm, int i, int j) {
@@ -290,7 +290,19 @@ __global__ void res_slots_kernel(double* __restrict__ rpk, const PulsarMeta* __r
       slot_val[rm.raw_off + i];
 }
 
-int upload_groups(const std::map<KernelCfg, std::vector<int>>& groups, std::vector<Group>* out) {
+bool PacketLayout::place(int p, int rows, PulsarMeta* pm) {
+  KernelCfg kc{};
+  if (!sweep_config(rows, &kc)) return false;
+  pm->ci = kc.ci;
+  pm->nch = (pm->n + kc.ci - 1) / kc.ci;
+  pm->mpad = kc.mp();
+  pm->pk_off = size;
+  size += (int64_t)pm->nch * pm->ci * (4 + pm->mpad);
+  groups[kc].push_back(p);
+  return true;
+}
+
+int PacketLayout::upload(std::vector<Group>* out) const {
   for (auto& kv : groups) {
     Group g;
     g.cfg = kv.first;
@@ -302,105 +314,97 @@ int upload_groups(const std::map<KernelCfg, std::vector<int>>& groups, std::vect
   return 0;
 }
 
-// the block-N side of build_res_packets: the arrays of bn on the device. The realisations go into (R, n_shared) blocks per
-// pulsar at R * smeta.raw_off, n_shared = min(pack, residual layout) TOAs: the two layouts agree position by position on
-// every real TOA (blockn.layout), so the pack's G rows and 1/N pair with them by position and the rest is padding.
-struct ResBlockNDev {
+// the arrays of a residual batch on the device. The realisations go into (R, n_shared) blocks per pulsar at
+// R * smeta.raw_off, n_shared = min(pack, residual layout) TOAs: the two layouts agree position by position on every real
+// TOA (blockn.layout; with a diagonal N they are the same layout), so the pack's G rows and 1/N pair with them by
+// position and the rest is padding. res_w is staged only when it is a separate array, the slot arrays only for block-N.
+struct ResDev {
   DeviceBuf<double> res, res_w, slot_val;
   DeviceBuf<int> slot_idx;
   DeviceBuf<PulsarMeta> smeta;  // the pack's meta with n = n_shared and raw_off into the (R, n_shared) blocks
 };
 
-static int stage_res_blockn(const ResBlockNHost& bn, int64_t R, const std::vector<PulsarMeta>& smeta,
-                            const std::vector<PulsarMeta>& rmeta, ResidualBatch* rb, ResBlockNDev* d, cudaStream_t st) {
+static int stage_res(const ResHost& h, int64_t R, bool blockn, const std::vector<PulsarMeta>& smeta,
+                     const std::vector<PulsarMeta>& rmeta, ResidualBatch* rb, ResDev* d, cudaStream_t st) {
   const int P = (int)smeta.size();
   const int64_t nsh = smeta.back().raw_off + smeta.back().n, nres = rmeta.back().raw_off + rmeta.back().n;
   const int64_t nchtot = rmeta.back().dm_off + rmeta.back().nch;
+  const bool sep_w = h.res_w != h.res;
   FFP_CUDA(dev_alloc(&d->res, (size_t)(R * nsh)));
-  FFP_CUDA(dev_alloc(&d->res_w, (size_t)(R * nsh)));
-  FFP_CUDA(dev_alloc(&d->slot_idx, (size_t)nres));
-  FFP_CUDA(dev_alloc(&d->slot_val, (size_t)nres));
-  FFP_CUDA(dev_alloc(&rb->done_mask, (size_t)nchtot));
+  if (sep_w) FFP_CUDA(dev_alloc(&d->res_w, (size_t)(R * nsh)));
+  if (blockn) {
+    FFP_CUDA(dev_alloc(&d->slot_idx, (size_t)nres));
+    FFP_CUDA(dev_alloc(&d->slot_val, (size_t)nres));
+    FFP_CUDA(dev_alloc(&rb->done_mask, (size_t)nchtot));
+  }
   FFP_CUDA(dev_alloc(&d->smeta, (size_t)P));
   FFP_CUDA(cudaMemcpyAsync(d->smeta.get(), smeta.data(), sizeof(PulsarMeta) * P, cudaMemcpyHostToDevice, st));
   for (int p = 0; p < P; ++p) {
     const PulsarMeta &sm = smeta[p], &rm = rmeta[p];
-    FFP_CUDA(cudaMemcpy2DAsync(d->res.get() + R * sm.raw_off, (size_t)sm.n * 8, bn.res[p], (size_t)rm.n * 8,
+    FFP_CUDA(cudaMemcpy2DAsync(d->res.get() + R * sm.raw_off, (size_t)sm.n * 8, h.res[p], (size_t)rm.n * 8,
                                (size_t)sm.n * 8, (size_t)R, cudaMemcpyHostToDevice, st));
-    FFP_CUDA(cudaMemcpy2DAsync(d->res_w.get() + R * sm.raw_off, (size_t)sm.n * 8, bn.res_w[p], (size_t)rm.n * 8,
-                               (size_t)sm.n * 8, (size_t)R, cudaMemcpyHostToDevice, st));
-    FFP_CUDA(cudaMemcpyAsync(d->slot_idx.get() + rm.raw_off, bn.slot_idx[p], (size_t)rm.n * sizeof(int),
+    if (sep_w)
+      FFP_CUDA(cudaMemcpy2DAsync(d->res_w.get() + R * sm.raw_off, (size_t)sm.n * 8, h.res_w[p], (size_t)rm.n * 8,
+                                 (size_t)sm.n * 8, (size_t)R, cudaMemcpyHostToDevice, st));
+    if (!blockn) continue;
+    FFP_CUDA(cudaMemcpyAsync(d->slot_idx.get() + rm.raw_off, h.slot_idx[p], (size_t)rm.n * sizeof(int),
                              cudaMemcpyHostToDevice, st));
-    FFP_CUDA(cudaMemcpyAsync(d->slot_val.get() + rm.raw_off, bn.slot_val[p], (size_t)rm.n * 8, cudaMemcpyHostToDevice,
+    FFP_CUDA(cudaMemcpyAsync(d->slot_val.get() + rm.raw_off, h.slot_val[p], (size_t)rm.n * 8, cudaMemcpyHostToDevice,
                              st));
-    FFP_CUDA(cudaMemcpyAsync(rb->done_mask.get() + rm.dm_off, bn.done_mask[p], (size_t)rm.nch, cudaMemcpyHostToDevice,
+    FFP_CUDA(cudaMemcpyAsync(rb->done_mask.get() + rm.dm_off, h.done_mask[p], (size_t)rm.nch, cudaMemcpyHostToDevice,
                              st));
   }
   return 0;
 }
 
-int build_res_packets(fastfp_pack* pk, int64_t R, const double* d_res, cudaStream_t st, const ResBlockNHost* bn) {
+int build_res_packets(fastfp_pack* pk, int64_t R, const ResHost& h, cudaStream_t st) {
   const int P = pk->P;
+  const bool blockn = pk->ecorr;
   std::vector<PulsarMeta> rmeta = pk->meta, smeta = pk->meta;
-  std::map<KernelCfg, std::vector<int>> groups;
-  int64_t off = 0, raw_off = 0, sh_off = 0, dm_off = 0;
+  PacketLayout lay;
+  int64_t raw_off = 0, sh_off = 0, dm_off = 0;
   int mmax = 0, nmax = 0, npad = 0;
   for (int p = 0; p < P; ++p) {
-    PulsarMeta& rm = rmeta[p];
-    KernelCfg kc{};
-    // block-N: the 8 epoch-slot rows after the realisations
-    if (!sweep_config((rm.m + 7) / 8 * 8 + (int)(R + 7) / 8 * 8 + (bn ? 8 : 0), &kc)) {
+    PulsarMeta &rm = rmeta[p], &sm = smeta[p];
+    rm.n = (int)h.n[p];
+    rm.raw_off = raw_off;
+    raw_off += rm.n;
+    sm.n = std::min(pk->meta[p].n, rm.n);
+    sm.raw_off = sh_off;
+    sh_off += sm.n;
+    if (!lay.place(p, sweep_rows(rm.m, R, blockn), &rm)) {
       set_error("residual batch: no kernel configuration for pulsar " + std::to_string(p));
-      return -3;
+      return FASTFP_ERR_UNSUPPORTED;
     }
-    if (bn) {
-      rm.n = (int)bn->n[p];
-      rm.raw_off = raw_off;
-      raw_off += rm.n;
-      rm.dm_off = dm_off;
-      dm_off += rm.n / kc.ci;
-      smeta[p].n = std::min(pk->meta[p].n, rm.n);
-      smeta[p].raw_off = sh_off;
-      sh_off += smeta[p].n;
-    }
-    rm.ci = kc.ci;
-    rm.nch = (rm.n + kc.ci - 1) / kc.ci;
-    rm.mpad = kc.mp();
-    rm.pk_off = off;
-    off += (int64_t)rm.nch * rm.ci * (4 + rm.mpad);
-    groups[kc].push_back(p);
+    rm.dm_off = dm_off;
+    dm_off += rm.nch;
     mmax = std::max(mmax, rm.m);
-    nmax = std::max(nmax, smeta[p].n);
+    nmax = std::max(nmax, sm.n);
     npad = std::max(npad, rm.nch * rm.ci);
   }
   ResidualBatch rb;
   FFP_CUDA(dev_alloc(&rb.meta, (size_t)P));
   FFP_CUDA(cudaMemcpy(rb.meta.get(), rmeta.data(), sizeof(PulsarMeta) * P, cudaMemcpyHostToDevice));
-  FFP_CUDA(dev_alloc(&rb.packets, (size_t)off));
-  if (int rc = upload_groups(groups, &rb.groups)) return rc;
-  rb.bytes = off * 8 + (int64_t)sizeof(PulsarMeta) * P + dm_off;
-  ResBlockNDev bd;
-  const PulsarMeta* d_smeta = pk->core.meta.get();  // diagonal N: the pack's own layout
-  const double* d_res_w = d_res;
-  if (bn) {
-    if (int rc = stage_res_blockn(*bn, R, smeta, rmeta, &rb, &bd, st)) return rc;
-    d_smeta = bd.smeta.get();
-    d_res = bd.res.get();
-    d_res_w = bd.res_w.get();  // the first term of w_k is N^-1 r_k, supplied as (N^-1 r_k) * Nvec (as in w_kernel)
-  }
+  FFP_CUDA(dev_alloc(&rb.packets, (size_t)lay.size));
+  if (int rc = lay.upload(&rb.groups)) return rc;
+  rb.bytes = lay.size * 8 + (int64_t)sizeof(PulsarMeta) * P + (blockn ? dm_off : 0);  // block-N: the slot masks
+  ResDev d;
+  if (int rc = stage_res(h, R, blockn, smeta, rmeta, &rb, &d, st)) return rc;
+  // the first term of w_k is N^-1 r_k, supplied as (N^-1 r_k) * Nvec (as in w_kernel): r_k itself for a diagonal N
+  const double* d_res_w = d.res_w ? d.res_w.get() : d.res.get();
   DeviceBuf<double> U;
   FFP_CUDA(dev_alloc(&U, (size_t)P * R * mmax));
   const PackCore& c = pk->core;
   res_packets_kernel<<<dim3((npad + 127) / 128, P), 128, 0, st>>>(rb.packets.get(), rb.meta.get(), c.packets.get(),
-                                                                  d_smeta);
-  ur_batch_kernel<<<dim3((mmax + 7) / 8, (unsigned)((R + 31) / 32), P), 256, 0, st>>>(c.packets.get(), d_smeta,
-                                                                                     d_res, (int)R, mmax, U.get());
+                                                                  d.smeta.get());
+  ur_batch_kernel<<<dim3((mmax + 7) / 8, (unsigned)((R + 31) / 32), P), 256, 0, st>>>(c.packets.get(), d.smeta.get(),
+                                                                                     d.res.get(), (int)R, mmax, U.get());
   w_batch_kernel<<<dim3((nmax + 31) / 32, (unsigned)((R + 7) / 8), P), 256, 0, st>>>(
-      rb.packets.get(), rb.meta.get(), c.packets.get(), d_smeta, d_res_w, (int)R, mmax, U.get());
+      rb.packets.get(), rb.meta.get(), c.packets.get(), d.smeta.get(), d_res_w, (int)R, mmax, U.get());
   g_launches += 3;
-  if (bn) {
-    res_slots_kernel<<<dim3((npad + 127) / 128, P), 128, 0, st>>>(rb.packets.get(), rb.meta.get(), bd.slot_idx.get(),
-                                                                  bd.slot_val.get());
+  if (blockn) {
+    res_slots_kernel<<<dim3((npad + 127) / 128, P), 128, 0, st>>>(rb.packets.get(), rb.meta.get(), d.slot_idx.get(),
+                                                                  d.slot_val.get());
     g_launches += 1;
   }
   FFP_CUDA(cudaGetLastError());

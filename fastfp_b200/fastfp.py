@@ -189,13 +189,12 @@ def batch_pass_rows(R: int, m, blockn: bool = False) -> int:
     ``m``: of the even splits of ``R`` into passes the library takes (at most ``_cabi.max_residual_rows`` rows each),
     the one with the least modelled cost, passes x :func:`_tile_cost` of ``roundup8(max m) + roundup8(rows)`` rows
     (``+ 8``, the epoch slots, for a block-diagonal N pack: ``blockn=True``); among equal costs the fewest passes."""
-    mr = -(-max(m) // 8) * 8 + (8 if blockn else 0)
     rmax = _cabi.max_residual_rows(m, blockn)
     best = None
     for cap in sorted({min(R, rmax)} | set(range(8, min(R, rmax), 8))):
         npass = -(-R // cap)
         rows = -(-R // npass)
-        cost = npass * _tile_cost(mr + -(-rows // 8) * 8)
+        cost = npass * _tile_cost(_cabi.sweep_rows(max(m), rows, blockn))
         if best is None or (cost, npass) < best[:2]:
             best = (cost, npass, rows)
     return best[2]
@@ -285,14 +284,7 @@ class FastFp(_PackCache):
         """Checks the shapes of ``residuals`` (a list of ``P`` arrays ``(R, n_p)``) and returns ``(R, passes)``:
         ``passes(pack, stream=0)`` yields the row ranges ``(lo, hi)`` of :func:`batch_pass_rows` passes with each
         pass's realisations set on ``pack``, uploaded again only when the pack or any byte of them changed."""
-        res = [_cabi.as_f64(r) for r in residuals]
-        if len(res) != len(self.toas):
-            raise ValueError(f"residuals must be a list of {len(self.toas)} arrays (one per pulsar)")
-        R = res[0].shape[0] if res[0].ndim == 2 else -1
-        for p, r in enumerate(res):
-            if r.shape != (R, self.toas[p].shape[0]):
-                raise ValueError(f"residuals[{p}] must have shape (R, {self.toas[p].shape[0]}) with the same R >= 1 for "
-                                 f"every pulsar; got {r.shape}")
+        res, R = _cabi.check_realisations(residuals, [t.shape[0] for t in self.toas])
         if R < 1:
             raise ValueError("residuals must hold at least one realisation")
         res_key = _fingerprint([res])
