@@ -21,6 +21,7 @@ c_double_pp = C.POINTER(c_double_p)
 FREQS_ON_DEVICE = 1
 OUT_ON_DEVICE = 2
 PARAMS_ON_DEVICE = 4
+SIM_NO_NOISE = 1
 
 # every symbol include/fastfp_b200.h declares: name -> (restype, argtypes)
 SYMBOLS = {
@@ -43,6 +44,17 @@ SYMBOLS = {
         C.c_int,
         [C.c_void_p, C.c_int64, c_int64_p, c_double_pp, c_double_pp, C.POINTER(C.POINTER(C.c_int32)), c_double_pp,
          C.POINTER(C.POINTER(C.c_ubyte)), C.c_void_p],
+    ),
+    "fastfp_pack_simulate_residuals": (
+        C.c_int,
+        [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, c_double_pp, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p],
+    ),
+    "fastfp_pack_simulate_residuals_blockn": (
+        C.c_int,
+        [C.c_void_p, C.c_int64, C.c_int64, C.c_int64, c_double_pp, C.c_void_p, C.c_void_p, c_int64_p,
+         C.POINTER(C.POINTER(C.c_int32)), c_double_pp, C.POINTER(C.POINTER(C.c_ubyte)),
+         C.POINTER(C.POINTER(C.c_int32)), C.POINTER(C.POINTER(C.c_int32)), c_double_pp, c_double_pp, C.c_int,
+         C.c_void_p],
     ),
     "fastfp_fp_sweep_residuals": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p]),
     "fastfp_fe_skymax_residuals": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64,
@@ -248,6 +260,7 @@ class Pack:
     def __init__(self, handle, P: int, device: int, nmfp: bool, n, m):
         self._h, self.P, self.device, self.nmfp = handle, P, device, nmfp
         self.n, self.m = list(n), list(m)
+        self._sim_layouts = {}  # block-N packs: simulate_residuals_blockn's layout arrays per tuple of chunk sizes
         self._warn_if_not_spd()
 
     PATHS = {"auto": 0, "fp64": 1, "i8": 2, "mixed": 3}
@@ -470,6 +483,76 @@ class Pack:
             self._h, R, _int64_array(n), _ptr_array(raw), _ptr_array(rw),
             i32pp(*[a.ctypes.data_as(C.POINTER(C.c_int32)) for a in sidx]), _ptr_array(sval),
             u8pp(*[a.ctypes.data_as(C.POINTER(C.c_ubyte)) for a in dm]), C.c_void_p(stream)))
+        self.R = R
+
+    def _sim_args(self, R, seed, first, phiinvs, signal, noise):
+        """The arguments both simulate calls share, checked: seed, first, the priors, the signal and the flags."""
+        from . import sim
+
+        seed, first = sim.check_seed(seed, first)
+        phi = sim.check_phiinvs(phiinvs, self.m)
+        freqs, amp = sim.signal_arrays(signal, R, self.P)
+        keep = (phi, freqs, amp)
+        args = (R, seed, first, _ptr_array(phi), None if freqs is None else _vp(freqs), None if amp is None else _vp(amp))
+        return args, (0 if noise else SIM_NO_NOISE), keep
+
+    def simulate_residuals(self, R: int, seed: int, phiinvs, first: int = 0, signal=None, noise: bool = True,
+                           stream: int = 0) -> None:
+        """:meth:`set_residuals` with ``R`` realisations of the pack's own noise model drawn on the device
+        (``fastfp_pack_simulate_residuals``): rows ``first .. first + R - 1`` of the stream of ``seed``, which
+        :func:`fastfp_b200.sim.simulate_residuals` reproduces on the host. ``phiinvs[p]`` is the ``(m_p,)`` prior
+        ``1/phi`` that went into ``sigma_p``; ``signal = (freqs, amp)`` as in :func:`fastfp_b200.sim.signal_arrays`;
+        ``noise=False`` sets the signal alone. ``R == 0`` releases the set."""
+        if self.blockn:
+            raise FastFpError("simulate_residuals needs a diagonal-N pack; this one has a block-diagonal N and takes "
+                              "simulate_residuals_blockn")
+        args, flags, keep = self._sim_args(R, seed, first, phiinvs, signal, noise)
+        check(load().fastfp_pack_simulate_residuals(self._h, *args, flags, C.c_void_p(stream)))
+        self.R = R
+
+    def simulate_residuals_blockn(self, R: int, seed: int, phiinvs, first: int = 0, signal=None, noise: bool = True,
+                                  stream: int = 0) -> None:
+        """:meth:`simulate_residuals` for a block-diagonal N pack (``fastfp_pack_simulate_residuals_blockn``): the
+        draw adds the ECORR epoch terms and the device applies the Sherman-Morrison ``N^-1``. The layout arrays of
+        :meth:`set_residuals_blockn` are built once per pulsar per call; nothing is done per realisation on the host."""
+        from . import blockn
+
+        if not self.blockn:
+            raise FastFpError("simulate_residuals_blockn needs a block-diagonal N pack; this one takes "
+                              "simulate_residuals")
+        args, flags, keep = self._sim_args(R, seed, first, phiinvs, signal, noise)
+        lib = load()
+        P = self.P
+        i32pp, u8pp = C.POINTER(C.c_int32) * P, C.POINTER(C.c_ubyte) * P
+        i32 = lambda arrs: i32pp(*[a.ctypes.data_as(C.POINTER(C.c_int32)) for a in arrs])  # noqa: E731
+        if R == 0 or R > max_residual_rows(self.m, blockn=True):  # nothing to lay out: the library releases or refuses
+            check(lib.fastfp_pack_simulate_residuals_blockn(self._h, *args, _int64_array(self.n), i32pp(),
+                                                            (c_double_p * P)(), u8pp(), i32pp(), i32pp(),
+                                                            (c_double_p * P)(), (c_double_p * P)(), flags,
+                                                            C.c_void_p(stream)))
+            self.R = 0
+            return
+        cis = tuple(lib.fastfp_sweep_chunk_toas(sweep_rows(m, R), 1) for m in self.m)
+        if cis not in self._sim_layouts:  # the layouts of these chunk sizes, kept for the next pass or call
+            arrs = [[] for _ in range(8)]
+            for ep, ci in zip(self.epochs, cis):
+                lay = blockn.layout(ep, ci)
+                order = lay["order"]
+                ep_of = np.full(ep.n, -1, dtype=np.int32)
+                for e, (a, b) in enumerate(ep.slices):
+                    ep_of[a:b] = e
+                eidx = np.where(order >= 0, ep_of[np.maximum(order, 0)], -1).astype(np.int32)
+                for lst, a in zip(arrs, (order.shape[0], lay["slot_idx"], lay["slot_val"], lay["done_mask"],
+                                         np.ascontiguousarray(order.astype(np.int32)), np.ascontiguousarray(eidx),
+                                         as_f64(np.sqrt(ep.jvec)) if ep.slices else np.zeros(1),
+                                         as_f64(ep.beta) if ep.slices else np.zeros(1))):
+                    lst.append(a)
+            self._sim_layouts[cis] = arrs
+        n, sidx, sval, dm, tidx, eidx, sj, beta = self._sim_layouts[cis]
+        check(lib.fastfp_pack_simulate_residuals_blockn(
+            self._h, *args, _int64_array(n), i32(sidx), _ptr_array(sval),
+            u8pp(*[a.ctypes.data_as(C.POINTER(C.c_ubyte)) for a in dm]), i32(tidx), i32(eidx), _ptr_array(sj),
+            _ptr_array(beta), flags, C.c_void_p(stream)))
         self.R = R
 
     def fp_sweep_residuals(self, freqs, out=None, stream: int = 0):

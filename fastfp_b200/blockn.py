@@ -86,12 +86,13 @@ def is_block(Nvec) -> bool:
 @dataclass
 class Epochs:
     """One pulsar's block-diagonal N as the layout and the Sherman-Morrison need it: the white variances ``nvec``,
-    the epochs ``slices`` as ``(start, stop)`` and ``beta_e = jvec_e / (1 + jvec_e * sum_e 1/nvec)``. A diagonal N
-    has no epochs."""
+    the epochs ``slices`` as ``(start, stop)``, ``beta_e = jvec_e / (1 + jvec_e * sum_e 1/nvec)`` and the epoch
+    variances ``jvec`` (what a draw of the noise needs). A diagonal N has no epochs."""
 
     nvec: np.ndarray
     slices: List[tuple]
     beta: np.ndarray
+    jvec: np.ndarray
 
     @property
     def n(self) -> int:
@@ -117,7 +118,7 @@ def epochs(Nvec, n: int) -> Epochs:
     if slices:
         idx, eid, offs = _epoch_index([slice(a, b) for a, b in slices])
         beta = jvec / (1.0 + jvec * np.add.reduceat(1.0 / nvec[idx], offs))
-    return Epochs(nvec, slices, beta)
+    return Epochs(nvec, slices, beta, jvec)
 
 
 def solve_rows(ep: Epochs, X) -> np.ndarray:

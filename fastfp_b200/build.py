@@ -18,7 +18,8 @@ INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 OUT_DIR = os.path.join(HERE, "_lib")
 LIB = os.path.join(OUT_DIR, "libfastfp_b200.so")
 SOURCES = ["cabi.cu", "precompute.cu", "fp_sweep.cu", "fp_sweep_w1.cu", "fp_sweep_w2.cu", "fp_sweep_w4.cu",
-           "fp_sweep_wide.cu", "fp_sweep_xwide.cu", "fp_sweep_i8.cu", "fe.cu", "nmfp.cu", "xcy.cu", "microbench.cu", "hostutil.cu"]
+           "fp_sweep_wide.cu", "fp_sweep_xwide.cu", "fp_sweep_i8.cu", "fe.cu", "nmfp.cu", "xcy.cu", "microbench.cu", "hostutil.cu",
+           "sim.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-fmad=true"]
 # developer builds only (e.g. FASTFP_B200_NVCC_FLAGS=-DFFP_DEBUG_SWITCHES for tools/dbg_split.sh); the

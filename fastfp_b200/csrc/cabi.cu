@@ -316,13 +316,35 @@ static int check_res_limit(const fastfp_pack* pk, int64_t R, const char* fn) {
 
 // Replaces the pack's residual batch with the R realisations of h (R == 0: none), once the sweeps queued on the stream,
 // which may still read the previous set, are done
-static int replace_res(fastfp_pack* pk, int64_t R, const ResHost& h, void* stream) {
+static int replace_res(fastfp_pack* pk, int64_t R, const ResHost& h, void* stream, const SimHost* sim = nullptr) {
   PackCall c(pk, stream);
   if (int rc = c.select()) return rc;
   FFP_CUDA(cudaStreamSynchronize(c.st));
   pk->res = {};
   if (R == 0) return FASTFP_OK;
-  return build_res_packets(pk, R, h, c.st);
+  return build_res_packets(pk, R, h, c.st, sim);
+}
+
+// The arguments both simulate entry points share (fastfp_pack_simulate_residuals*): FASTFP_ERR_INVALID for a negative
+// seed or first index, a signal given by half, an unknown flag, or a prior that is not finite and >= 0
+static int check_sim_args(const fastfp_pack* pk, int64_t R, int64_t seed, int64_t first, const double* const* phiinv,
+                          const double* sig_freq, const double* sig_amp, int flags, const char* fn) {
+  if (seed < 0 || first < 0 || first > INT64_MAX - R || (!sig_freq != !sig_amp) || (flags & ~FASTFP_SIM_NO_NOISE)) {
+    set_error(std::string(fn) + ": seed and first must be >= 0, sig_freq and sig_amp both given or both NULL, and "
+              "flags 0 or FASTFP_SIM_NO_NOISE");
+    return FASTFP_ERR_INVALID;
+  }
+  for (int p = 0; p < pk->P && R > 0; ++p) {
+    if (!phiinv[p]) { set_error(std::string(fn) + ": null per-pulsar array"); return FASTFP_ERR_INVALID; }
+    for (int j = 0; j < pk->meta[p].m; ++j) {
+      if (!(phiinv[p][j] >= 0.0) || !std::isfinite(phiinv[p][j])) {
+        set_error(std::string(fn) + ": pulsar " + std::to_string(p) + ": phiinv[" + std::to_string(j) +
+                  "] must be finite and >= 0");
+        return FASTFP_ERR_INVALID;
+      }
+    }
+  }
+  return FASTFP_OK;
 }
 
 }  // namespace ffp
@@ -517,6 +539,77 @@ int fastfp_pack_set_residuals_blockn(fastfp_pack_t* pk, int64_t R, const int64_t
     }
   }
   return replace_res(pk, R, {n, residuals, residuals_w, slot_idx, slot_val, done_mask}, stream);
+}
+
+// Residual batches drawn on the device (DESIGN.md section 5g): the staging that set_residuals fills from the host is
+// filled by sim_noise_kernel, and sim_basis_kernel adds the basis draw between G n and w
+int fastfp_pack_simulate_residuals(fastfp_pack_t* pk, int64_t R, int64_t seed, int64_t first,
+                                   const double* const* phiinv, const double* sig_freq, const double* sig_amp,
+                                   int flags, void* stream) {
+  if (!pk || R < 0 || (R > 0 && !phiinv)) {
+    set_error("fastfp_pack_simulate_residuals: null argument or negative R");
+    return FASTFP_ERR_INVALID;
+  }
+  if (pk->nmfp) {
+    set_error("fastfp_pack_simulate_residuals needs a plain-Fp pack (fastfp_pack_create)");
+    return FASTFP_ERR_INVALID;
+  }
+  if (pk->ecorr) {
+    set_error("fastfp_pack_simulate_residuals: a block-diagonal N pack takes its realisations in its own TOA layout "
+              "(fastfp_pack_simulate_residuals_blockn)");
+    return FASTFP_ERR_UNSUPPORTED;
+  }
+  const char* fn = "fastfp_pack_simulate_residuals";
+  if (int rc = check_sim_args(pk, R, seed, first, phiinv, sig_freq, sig_amp, flags, fn)) return rc;
+  if (int rc = check_res_limit(pk, R, fn)) return rc;
+  std::vector<int64_t> n(pk->P);
+  for (int p = 0; p < pk->P; ++p) n[p] = pk->meta[p].n;
+  const SimHost sim{seed, first, !(flags & FASTFP_SIM_NO_NOISE), phiinv, sig_freq, sig_amp,
+                    nullptr, nullptr, nullptr, nullptr};
+  return replace_res(pk, R, {n.data(), nullptr, nullptr, nullptr, nullptr, nullptr}, stream, &sim);
+}
+
+int fastfp_pack_simulate_residuals_blockn(fastfp_pack_t* pk, int64_t R, int64_t seed, int64_t first,
+                                          const double* const* phiinv, const double* sig_freq, const double* sig_amp,
+                                          const int64_t* n, const int32_t* const* slot_idx,
+                                          const double* const* slot_val, const unsigned char* const* done_mask,
+                                          const int32_t* const* toa_index, const int32_t* const* epoch,
+                                          const double* const* sqrt_j, const double* const* beta, int flags,
+                                          void* stream) {
+  if (!pk || R < 0 ||
+      (R > 0 && (!phiinv || !n || !slot_idx || !slot_val || !done_mask || !toa_index || !epoch || !sqrt_j || !beta))) {
+    set_error("fastfp_pack_simulate_residuals_blockn: null argument or negative R");
+    return FASTFP_ERR_INVALID;
+  }
+  if (pk->nmfp) {
+    set_error("fastfp_pack_simulate_residuals_blockn needs a plain-Fp pack (fastfp_pack_create_blockn without m_fix)");
+    return FASTFP_ERR_INVALID;
+  }
+  if (!pk->ecorr) {
+    set_error("fastfp_pack_simulate_residuals_blockn needs a block-diagonal N pack; a diagonal-N pack takes "
+              "fastfp_pack_simulate_residuals");
+    return FASTFP_ERR_INVALID;
+  }
+  const char* fn = "fastfp_pack_simulate_residuals_blockn";
+  if (int rc = check_sim_args(pk, R, seed, first, phiinv, sig_freq, sig_amp, flags, fn)) return rc;
+  if (int rc = check_res_limit(pk, R, fn)) return rc;
+  for (int p = 0; p < pk->P && R > 0; ++p) {
+    if (!slot_idx[p] || !slot_val[p] || !done_mask[p] || !toa_index[p] || !epoch[p] || !sqrt_j[p] || !beta[p]) {
+      set_error(std::string(fn) + ": null per-pulsar array");
+      return FASTFP_ERR_INVALID;
+    }
+    KernelCfg kc{};
+    if (!sweep_config(sweep_rows(pk->meta[p].m, R, true), &kc) || n[p] < 1 || n[p] > 0x7fffff00LL ||
+        n[p] % kc.ci != 0) {
+      set_error(std::string(fn) + ": pulsar " + std::to_string(p) + ": the TOA count " + std::to_string(n[p]) +
+                " of the residual layout must be a positive multiple of its chunk size " + std::to_string(kc.ci) +
+                " (fastfp_sweep_chunk_toas(roundup8(m) + roundup8(R), 1))");
+      return FASTFP_ERR_INVALID;
+    }
+  }
+  const SimHost sim{seed, first, !(flags & FASTFP_SIM_NO_NOISE), phiinv, sig_freq, sig_amp,
+                    toa_index, epoch, sqrt_j, beta};
+  return replace_res(pk, R, {n, nullptr, nullptr, slot_idx, slot_val, done_mask}, stream, &sim);
 }
 
 int fastfp_fp_sweep_residuals(const fastfp_pack_t* pk, const double* freqs, int64_t F, double* out, int flags,

@@ -332,8 +332,57 @@ struct ResHost {
   const double* const* slot_val;
   const unsigned char* const* done_mask;
 };
-// the residual packets of R realisations into pk->res, which the caller has released
-int build_res_packets(fastfp_pack* pk, int64_t R, const ResHost& h, cudaStream_t st);
+// a residual batch drawn on the device (sim.cu, DESIGN.md section 5g): the stream's seed and first realisation index,
+// per pulsar the prior phiinv (m_p), the signal (sig_freq (R), sig_amp (R, P, 2); both null: none); block-N packs also
+// per position of the residual layout the original TOA index and the epoch (-1: none), per epoch sqrt(j_e) and beta_e
+struct SimHost {
+  int64_t seed, first;
+  bool noise;
+  const double* const* phiinv;
+  const double* sig_freq;
+  const double* sig_amp;
+  const int32_t* const* toa_index;
+  const int32_t* const* epoch;
+  const double* const* sqrt_j;
+  const double* const* beta;
+};
+// its device side
+struct SimArgs {
+  uint64_t seed, first;
+  int noise;
+  const double* sig_freq;  // (R) or null: no signal
+  const double* sig_amp;   // (R, P, 2): (A_s, A_c)
+  const double* phiinv;    // [P][MAX_M]
+  // block-diagonal N (all null for a diagonal N): per position of the (R, n_shared) staging at smeta.raw_off the
+  // original TOA index (-1 on padding); the segments, nseg_p + 1 starts per pulsar from seg_off[p] (an epoch's run of
+  // positions, or one position outside any epoch), and each one's epoch; per epoch sqrt(j_e) and beta_e from ep_off[p]
+  const int* toa_index;
+  const int* seg;
+  const int* seg_epoch;
+  const int64_t* seg_off;
+  const double* sqrt_j;
+  const double* beta;
+  const int64_t* ep_off;
+};
+// the device arrays of SimArgs and the host arrays their copies read, held until the batch is built
+struct SimStage {
+  SimArgs args{};
+  DeviceBuf<double> phiinv, sig_freq, sig_amp, sqrt_j, beta;
+  DeviceBuf<int> toa_index, seg, seg_epoch;
+  DeviceBuf<int64_t> seg_off, ep_off;
+  std::vector<double> host_phi, host_sqrt_j, host_beta;
+  std::vector<int> host_idx, host_seg, host_seg_ep;
+  std::vector<int64_t> host_seg_off, host_ep_off;
+};
+// sim_noise_kernel: the realisations n_k into the (R, n_shared) staging (and res_w for a block N)
+int launch_sim_noise(const SimHost& s, const fastfp_pack* pk, const std::vector<PulsarMeta>& smeta,
+                     const PulsarMeta* d_smeta, int64_t R, double* d_res, double* d_res_w, SimStage* ss,
+                     cudaStream_t st);
+// sim_basis_kernel: U[p][k] -= L^-1 (sqrt(phiinv) o zeta), U as ur_batch_kernel writes it (row stride ld)
+int launch_sim_basis(const fastfp_pack* pk, int64_t R, double* d_U, int ld, const SimStage& ss, cudaStream_t st);
+// the residual packets of R realisations into pk->res, which the caller has released: uploaded from h.res / h.res_w, or
+// drawn on the device when sim is set (h then gives the layout only)
+int build_res_packets(fastfp_pack* pk, int64_t R, const ResHost& h, cudaStream_t st, const SimHost* sim = nullptr);
 // packets of pulsars one after another, each in the kernel configuration for its number of G rows
 struct PacketLayout {
   int64_t size = 0;                              // doubles

@@ -318,18 +318,19 @@ int PacketLayout::upload(std::vector<Group>* out) const {
 // R * smeta.raw_off, n_shared = min(pack, residual layout) TOAs: the two layouts agree position by position on every real
 // TOA (blockn.layout; with a diagonal N they are the same layout), so the pack's G rows and 1/N pair with them by
 // position and the rest is padding. res_w is staged only when it is a separate array, the slot arrays only for block-N.
+// A simulated batch gets the same blocks, left for sim_noise_kernel to fill.
 struct ResDev {
   DeviceBuf<double> res, res_w, slot_val;
   DeviceBuf<int> slot_idx;
   DeviceBuf<PulsarMeta> smeta;  // the pack's meta with n = n_shared and raw_off into the (R, n_shared) blocks
 };
 
-static int stage_res(const ResHost& h, int64_t R, bool blockn, const std::vector<PulsarMeta>& smeta,
+static int stage_res(const ResHost& h, bool simulated, int64_t R, bool blockn, const std::vector<PulsarMeta>& smeta,
                      const std::vector<PulsarMeta>& rmeta, ResidualBatch* rb, ResDev* d, cudaStream_t st) {
   const int P = (int)smeta.size();
   const int64_t nsh = smeta.back().raw_off + smeta.back().n, nres = rmeta.back().raw_off + rmeta.back().n;
   const int64_t nchtot = rmeta.back().dm_off + rmeta.back().nch;
-  const bool sep_w = h.res_w != h.res;
+  const bool sep_w = simulated ? blockn : h.res_w != h.res;
   FFP_CUDA(dev_alloc(&d->res, (size_t)(R * nsh)));
   if (sep_w) FFP_CUDA(dev_alloc(&d->res_w, (size_t)(R * nsh)));
   if (blockn) {
@@ -341,9 +342,10 @@ static int stage_res(const ResHost& h, int64_t R, bool blockn, const std::vector
   FFP_CUDA(cudaMemcpyAsync(d->smeta.get(), smeta.data(), sizeof(PulsarMeta) * P, cudaMemcpyHostToDevice, st));
   for (int p = 0; p < P; ++p) {
     const PulsarMeta &sm = smeta[p], &rm = rmeta[p];
-    FFP_CUDA(cudaMemcpy2DAsync(d->res.get() + R * sm.raw_off, (size_t)sm.n * 8, h.res[p], (size_t)rm.n * 8,
-                               (size_t)sm.n * 8, (size_t)R, cudaMemcpyHostToDevice, st));
-    if (sep_w)
+    if (!simulated)
+      FFP_CUDA(cudaMemcpy2DAsync(d->res.get() + R * sm.raw_off, (size_t)sm.n * 8, h.res[p], (size_t)rm.n * 8,
+                                 (size_t)sm.n * 8, (size_t)R, cudaMemcpyHostToDevice, st));
+    if (sep_w && !simulated)
       FFP_CUDA(cudaMemcpy2DAsync(d->res_w.get() + R * sm.raw_off, (size_t)sm.n * 8, h.res_w[p], (size_t)rm.n * 8,
                                  (size_t)sm.n * 8, (size_t)R, cudaMemcpyHostToDevice, st));
     if (!blockn) continue;
@@ -357,7 +359,7 @@ static int stage_res(const ResHost& h, int64_t R, bool blockn, const std::vector
   return 0;
 }
 
-int build_res_packets(fastfp_pack* pk, int64_t R, const ResHost& h, cudaStream_t st) {
+int build_res_packets(fastfp_pack* pk, int64_t R, const ResHost& h, cudaStream_t st, const SimHost* sim) {
   const int P = pk->P;
   const bool blockn = pk->ecorr;
   std::vector<PulsarMeta> rmeta = pk->meta, smeta = pk->meta;
@@ -389,7 +391,11 @@ int build_res_packets(fastfp_pack* pk, int64_t R, const ResHost& h, cudaStream_t
   if (int rc = lay.upload(&rb.groups)) return rc;
   rb.bytes = lay.size * 8 + (int64_t)sizeof(PulsarMeta) * P + (blockn ? dm_off : 0);  // block-N: the slot masks
   ResDev d;
-  if (int rc = stage_res(h, R, blockn, smeta, rmeta, &rb, &d, st)) return rc;
+  if (int rc = stage_res(h, sim != nullptr, R, blockn, smeta, rmeta, &rb, &d, st)) return rc;
+  SimStage ss;
+  if (sim) {
+    if (int rc = launch_sim_noise(*sim, pk, smeta, d.smeta.get(), R, d.res.get(), d.res_w.get(), &ss, st)) return rc;
+  }
   // the first term of w_k is N^-1 r_k, supplied as (N^-1 r_k) * Nvec (as in w_kernel): r_k itself for a diagonal N
   const double* d_res_w = d.res_w ? d.res_w.get() : d.res.get();
   DeviceBuf<double> U;
@@ -399,6 +405,10 @@ int build_res_packets(fastfp_pack* pk, int64_t R, const ResHost& h, cudaStream_t
                                                                   d.smeta.get());
   ur_batch_kernel<<<dim3((mmax + 7) / 8, (unsigned)((R + 31) / 32), P), 256, 0, st>>>(c.packets.get(), d.smeta.get(),
                                                                                      d.res.get(), (int)R, mmax, U.get());
+  // simulated: U = G n - L^-1 (sqrt(phiinv) o zeta), which turns w into C^-1 (n + T Phi^(1/2) zeta) (DESIGN.md 5g)
+  if (sim && sim->noise) {
+    if (int rc = launch_sim_basis(pk, R, U.get(), mmax, ss, st)) return rc;
+  }
   w_batch_kernel<<<dim3((nmax + 31) / 32, (unsigned)((R + 7) / 8), P), 256, 0, st>>>(
       rb.packets.get(), rb.meta.get(), c.packets.get(), d.smeta.get(), d_res_w, (int)R, mmax, U.get());
   g_launches += 3;

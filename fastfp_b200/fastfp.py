@@ -280,29 +280,86 @@ class FastFp(_PackCache):
 
         return self._run_verified((Nvecs, Ts, sigmas), run, asynchronous=on_device).reshape((R,) + np.shape(fgw))
 
+    def calculate_Fp_simulated(self, fgw, Nvecs, Ts, sigmas, phiinvs, R, seed, first=0, signal=None, noise=True):
+        """:meth:`calculate_Fp_batch` on ``R`` realisations of the noise model of ``Nvecs, Ts, sigmas`` drawn on the
+        device: row ``k`` is realisation ``first + k`` of the stream of ``seed``, the residuals ``n + T Phi^(1/2)
+        zeta`` (white noise, ECORR epoch terms for a block-diagonal N, the basis with prior ``1/phiinvs``) plus an
+        optional Earth-term signal. Nothing is drawn or uploaded per realisation on the host
+        (``fastfp_pack_simulate_residuals``; DESIGN.md section 5g). :func:`fastfp_b200.sim.simulate_residuals` gives
+        the same realisations on the host.
+
+        ``phiinvs[p]`` is the ``(m_p,)`` prior ``1/phi`` that went into ``sigmas[p]`` (``pta.get_phiinv``); ``seed``
+        and ``first`` are integers ``>= 0``. ``signal = (freqs, amp)``: ``freqs`` a scalar or ``(R,)``, ``amp``
+        ``(P, 2)`` or ``(R, P, 2)``, each pulsar's ``(A_s, A_c)`` of ``A_s sin(2 pi f t) + A_c cos(2 pi f t)``
+        (:meth:`FastFe.cw_signal` builds it from the Fe amplitudes); ``noise=False`` sweeps the signal alone. The
+        result has the shape and device semantics of :meth:`calculate_Fp_batch`, and is computed in passes of
+        :func:`batch_pass_rows` rows the same way; a realisation is the same whatever ``R``, ``first`` or pass split
+        drew it."""
+        R, passes = self._simulated_passes(Ts, phiinvs, R, seed, first, signal, noise)
+        f, empty, stream, on_device = self._front_end(fgw)
+        out = empty((R, f.shape[0]))
+
+        def run(pack):
+            for lo, hi in passes(pack, stream):
+                pack.fp_sweep_residuals(f, out=out[lo:hi], stream=stream)
+            return out
+
+        return self._run_verified((Nvecs, Ts, sigmas), run, asynchronous=on_device).reshape((R,) + np.shape(fgw))
+
     def _residual_passes(self, residuals):
-        """Checks the shapes of ``residuals`` (a list of ``P`` arrays ``(R, n_p)``) and returns ``(R, passes)``:
-        ``passes(pack, stream=0)`` yields the row ranges ``(lo, hi)`` of :func:`batch_pass_rows` passes with each
-        pass's realisations set on ``pack``, uploaded again only when the pack or any byte of them changed."""
+        """Checks the shapes of ``residuals`` (a list of ``P`` arrays ``(R, n_p)``) and returns ``(R, passes)`` of
+        :meth:`_passes` that upload them."""
         res, R = _cabi.check_realisations(residuals, [t.shape[0] for t in self.toas])
         if R < 1:
             raise ValueError("residuals must hold at least one realisation")
-        res_key = _fingerprint([res])
+
+        def upload(pack, lo, hi, stream):
+            fn = pack.set_residuals_blockn if getattr(pack, "blockn", False) else pack.set_residuals
+            fn([r[lo:hi] for r in res], stream=stream)
+
+        return R, self._passes(R, ("uploaded", _fingerprint([res])), upload)
+
+    def _simulated_passes(self, Ts, phiinvs, R, seed, first, signal, noise):
+        """Checks the arguments of a simulated batch and returns ``(R, passes)`` of :meth:`_passes` that draw it."""
+        from . import sim
+
+        if isinstance(R, (bool, np.bool_)) or not isinstance(R, (int, np.integer)) or R < 1:
+            raise ValueError("R must be an integer >= 1")
+        R = int(R)
+        seed, first = sim.check_seed(seed, first)
+        if first > 2 ** 63 - 1 - R:
+            raise ValueError("first + R must stay below 2^63")
+        if len(Ts) != len(self.toas):
+            raise ValueError(f"Ts must be a list of {len(self.toas)} arrays (one per pulsar)")
+        phi = sim.check_phiinvs(phiinvs, [np.shape(T)[1] for T in Ts])
+        freqs, amp = sim.signal_arrays(signal, R, len(self.toas))
+        sig = [] if freqs is None else [freqs, amp]
+        key = ("simulated", seed, first, bool(noise), freqs is None, _fingerprint([phi, sig]))
+
+        def upload(pack, lo, hi, stream):
+            fn = pack.simulate_residuals_blockn if getattr(pack, "blockn", False) else pack.simulate_residuals
+            part = None if freqs is None else (freqs[lo:hi], amp[lo:hi])
+            fn(hi - lo, seed, phi, first=first + lo, signal=part, noise=noise, stream=stream)
+
+        return R, self._passes(R, key, upload)
+
+    def _passes(self, R, key, upload):
+        """``passes(pack, stream=0)`` yields the row ranges ``(lo, hi)`` of :func:`batch_pass_rows` passes with each
+        pass's realisations set on ``pack`` by ``upload(pack, lo, hi, stream)``, again only when the pack or ``key``
+        (the content of the set: an uploaded set and a simulated set never share one) changed."""
 
         def passes(pack, stream=0):
             blockn = getattr(pack, "blockn", False)  # a pack without the attribute has a diagonal N
             rows = batch_pass_rows(R, pack.m, blockn)
-            upload = pack.set_residuals_blockn if blockn else pack.set_residuals
             for lo in range(0, R, rows):
                 hi = min(R, lo + rows)
-                key = (res_key, lo, hi)
-                if self._res_pack is not pack or self._res_key != key:
+                if self._res_pack is not pack or self._res_key != (key, lo, hi):
                     self._res_pack, self._res_key = None, None
-                    upload([r[lo:hi] for r in res], stream=stream)
-                    self._res_pack, self._res_key = pack, key
+                    upload(pack, lo, hi, stream)
+                    self._res_pack, self._res_key = pack, (key, lo, hi)
                 yield lo, hi
 
-        return R, passes
+        return passes
 
     _res_pack = None
     _res_key = None

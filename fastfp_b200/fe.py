@@ -91,6 +91,19 @@ class FastFe(FastFp):
         the ``Nvecs`` works as in :meth:`calculate_Fp_batch`."""
         fplus, fcross = self._sky_grid(gwtheta, gwphi)
         R, passes = self._residual_passes(residuals)
+        return self._skymax_passes(fgw, fplus, fcross, Nvecs, Ts, sigmas, R, passes)
+
+    def calculate_Fe_skymax_simulated(self, fgw, gwtheta, gwphi, Nvecs, Ts, sigmas, phiinvs, R, seed, first=0,
+                                      signal=None, noise=True):
+        """:meth:`calculate_Fe_skymax_batch` on ``R`` realisations of the noise model drawn on the device, with the
+        arguments, stream and signal of :meth:`calculate_Fp_simulated`: the all-sky scan of simulated noise that
+        calibrates the search's false-alarm threshold, or of injected signals (:meth:`cw_signal`) for its detection
+        probability. Returns ``(fe_max, sky_index)`` shaped as for :meth:`calculate_Fe_skymax_batch`."""
+        fplus, fcross = self._sky_grid(gwtheta, gwphi)
+        R, passes = self._simulated_passes(Ts, phiinvs, R, seed, first, signal, noise)
+        return self._skymax_passes(fgw, fplus, fcross, Nvecs, Ts, sigmas, R, passes)
+
+    def _skymax_passes(self, fgw, fplus, fcross, Nvecs, Ts, sigmas, R, passes):
         f, empty, stream, on_device = self._front_end(fgw)
         best, idx = empty((R, f.shape[0])), empty((R, f.shape[0]), np.int64)
 
@@ -102,6 +115,22 @@ class FastFe(FastFp):
         best, idx = self._run_verified((Nvecs, Ts, sigmas), run, asynchronous=on_device)
         shape = (R,) + np.shape(fgw)
         return best.reshape(shape), idx.reshape(shape)
+
+    def cw_signal(self, fgw, gwtheta, gwphi, a):
+        """The ``signal`` argument of :meth:`calculate_Fp_simulated` / :meth:`calculate_Fe_skymax_simulated` for an
+        Earth-term source at frequency ``fgw`` (scalar or ``(R,)``) and sky position ``(gwtheta, gwphi)`` with the four
+        Fe amplitudes ``a`` (``(4,)`` or ``(R, 4)``), the coefficients of the templates ``[F+ s, F+ c, Fx s, Fx c]``:
+        ``A_s = a1 F+ + a3 Fx`` and ``A_c = a2 F+ + a4 Fx`` per pulsar (:func:`antenna_pattern`). Returns ``(fgw,
+        amp)`` with ``amp`` ``(P, 2)`` or ``(R, P, 2)``."""
+        a = np.asarray(a, dtype=np.float64)
+        if a.shape[-1:] != (4,) or a.ndim > 2:
+            raise ValueError("a must have shape (4,) or (R, 4)")
+        fplus, fcross = antenna_pattern(self.pos, gwtheta, gwphi)
+        if np.ndim(fplus) != 1:
+            raise ValueError("cw_signal takes one sky position")
+        a = a[..., None, :]
+        amp = np.stack((a[..., 0] * fplus + a[..., 2] * fcross, a[..., 1] * fplus + a[..., 3] * fcross), axis=-1)
+        return np.asarray(fgw, dtype=np.float64), amp
 
     def _sky_grid(self, gwtheta, gwphi):
         """Antenna patterns ``(F+, Fx)``, each ``(S, P)``, of the sky grid ``gwtheta``, ``gwphi`` broadcast to ``(S,)``."""

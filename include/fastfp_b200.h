@@ -165,6 +165,55 @@ int fastfp_pack_set_residuals_blockn(fastfp_pack_t* pack, int64_t R, const int64
                                      const double* const* residuals_w, const int32_t* const* slot_idx,
                                      const double* const* slot_val, const unsigned char* const* done_mask,
                                      void* stream);
+/* ---- residual batches drawn on the device (DESIGN.md section 5g) -------------------------------------------
+ * fastfp_pack_simulate_residuals: sets R realisations r_k = n_k + T Phi^(1/2) zeta_k (+ s_k) of the pack's own noise
+ *   model, drawn on the device, as fastfp_pack_set_residuals would set them from the host, for
+ *   fastfp_fp_sweep_residuals and fastfp_fe_skymax_residuals. n_k is the white noise sqrt(N_i) z_i, zeta_k the basis
+ *   draw, s_k the optional Earth-term signal A_s[k,p] sin(((2 pi) f_k) t) + A_c[k,p] cos(((2 pi) f_k) t), the template
+ *   of the sweep, phase rounding and sincos rule included. The realisations are never formed: with w = C^-1 r and
+ *   C^-1 T Phi = N^-1 T Sigma^-1 the sweep needs w_k = N^-1 n_k - G^T (G n_k - L^-1 (sqrt(phiinv) o zeta_k)) with the
+ *   pack's G and Sigma = L L^T, so the draw has covariance exactly N + T Phi T^T = C, timing-model columns included
+ *   (phiinv = 1e-40 gives them a negligible weight; phiinv = 0, a flat prior, contributes nothing).
+ *     seed     >= 0; first >= 0: the global index of the first realisation (row k is realisation first + k)
+ *     phiinv[p] host array (m_p): the 1/phi that went into sigma_p; finite and >= 0
+ *     sig_freq host array (R) and sig_amp host array (R, P, 2) of (A_s, A_c), or both NULL: no signal
+ *     flags    0, or FASTFP_SIM_NO_NOISE: the signal alone
+ *   Random stream: Philox4x64-10 with key (seed, 0) and counter (q, k, p, tag), k = first + row the global realisation
+ *   index, p the pulsar, tag 0 for the white noise (normal number = the pulsar's original TOA index), 1 for the ECORR
+ *   epoch draws of fastfp_pack_simulate_residuals_blockn (normal number = epoch, in the caller's slice order) and 2
+ *   for the basis columns (normal number = column j). Counter block q gives normals 4q .. 4q+3: each of its four
+ *   64-bit words x becomes the uniform ((x >> 11) + 0.5) 2^-53 in (0, 1] (never 0; the largest word rounds to
+ *   1), and Box-Muller maps (u0, u1) to
+ *   sqrt(-2 ln u0) (cos, sin)(2 pi u1) and (u2, u3) likewise. So realisation k is the same whatever R, first or pass
+ *   split produced it; np.random.Philox(key=[seed, 0], counter=[q - 1, k, p, tag]).random_raw(4) gives block q, q >= 1
+ *   (fastfp_b200/sim.py is the host reference).
+ *   Limits, the R == 0 release, the refusal of an nmfp pack (FASTFP_ERR_INVALID) and of a block-N pack
+ *   (FASTFP_ERR_UNSUPPORTED) as for fastfp_pack_set_residuals; FASTFP_ERR_INVALID also for a negative seed or first,
+ *   a signal given by half, an unknown flag or a phiinv entry that is negative or not finite. Device staging as for
+ *   fastfp_pack_set_residuals: R * sum_p n_p doubles, freed before it returns; the R x m draws of the basis need no
+ *   more, and nothing crosses PCIe per realisation but the signal (3 P + 1 doubles). */
+#define FASTFP_SIM_NO_NOISE 1
+int fastfp_pack_simulate_residuals(fastfp_pack_t* pack, int64_t R, int64_t seed, int64_t first,
+                                   const double* const* phiinv, const double* sig_freq, const double* sig_amp,
+                                   int flags, void* stream);
+/* fastfp_pack_simulate_residuals_blockn: the same for a block-diagonal N pack, whose n_k also holds the ECORR draws
+ *   sqrt(j_e) eta_e on every TOA of epoch e, and whose N^-1 n_k is applied on the device (Sherman-Morrison). n,
+ *   slot_idx, slot_val and done_mask are the residual layout of fastfp_pack_set_residuals_blockn; per pulsar also
+ *     toa_index[p]  per position of that layout, the original TOA index (-1 on padding)
+ *     epoch[p]      per position, the epoch (index into the caller's slices; -1 outside any epoch and on padding);
+ *                   every epoch one contiguous run of positions
+ *     sqrt_j[p], beta[p]  per epoch: sqrt(j_e) and beta_e = j_e / (1 + j_e sum_e 1/Nvec)
+ *   Refusals as for fastfp_pack_set_residuals_blockn plus those of fastfp_pack_simulate_residuals, and
+ *   FASTFP_ERR_INVALID for an epoch or TOA index out of range, an epoch split in two runs, or a sqrt_j / beta that is
+ *   not finite (sqrt_j < 0). Device staging: 2 R * sum_p n_p doubles (n_k and (N^-1 n_k) * Nvec), freed before it
+ *   returns, as for fastfp_pack_set_residuals_blockn. */
+int fastfp_pack_simulate_residuals_blockn(fastfp_pack_t* pack, int64_t R, int64_t seed, int64_t first,
+                                          const double* const* phiinv, const double* sig_freq, const double* sig_amp,
+                                          const int64_t* n, const int32_t* const* slot_idx,
+                                          const double* const* slot_val, const unsigned char* const* done_mask,
+                                          const int32_t* const* toa_index, const int32_t* const* epoch,
+                                          const double* const* sqrt_j, const double* const* beta, int flags,
+                                          void* stream);
 int fastfp_fp_sweep_residuals(const fastfp_pack_t* pack, const double* freqs, int64_t F, double* out, int flags,
                               void* stream);
 
