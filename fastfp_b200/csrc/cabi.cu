@@ -930,7 +930,7 @@ int fastfp_tnt(int device, int64_t n, int64_t m, const double* Nvec, const doubl
 }
 
 int fastfp_fp64_peak(int device, int kind, int iters, double* tflops, double* ms) {
-  if (!tflops || !ms || iters < 1 || kind < 0 || kind > 24) {
+  if (!tflops || !ms || iters < 1 || kind < 0 || kind > 25) {
     set_error("fastfp_fp64_peak: invalid argument");
     return FASTFP_ERR_INVALID;
   }

@@ -17,11 +17,10 @@ namespace ffp {
 
 // ---- tiling constants of the sweep kernel (DESIGN.md section 4) -------------------------
 constexpr int NWC = 8;         // consumer (MMA) warps per sweep CTA: two per SM sub-partition
-constexpr int NWP = 16;        // producer (sincos) warps per sweep CTA: four per SM sub-partition
+constexpr int NWP = 16;        // producer (sincos) warps per sweep CTA by default: four per SM sub-partition
 constexpr int NTC = NWC * 32, NTP = NWP * 32;
-constexpr int NTHREADS = NTC + NTP;  // 768 threads per sweep CTA, one CTA per SM
 constexpr int CTAS_PER_SM = 1;
-constexpr int CONSUMER_REGS = 120, PRODUCER_REGS = 56;  // setmaxnreg split of the 768 x 80 pool
+constexpr int CONSUMER_REGS = 120, PRODUCER_REGS = 56;  // default setmaxnreg split of the 768 x 80 pool
 constexpr int VST = 16;        // TOA-vector ring depth (t | 1/N | w; TMA -> producer)
 constexpr int FLUSH_TOAS = 512;  // level-1 accumulation block, in TOAs
 constexpr int MAX_M = 640;     // widest basis the sweep kernel handles (8 warp rows x 10 blocks of 8 rows)
@@ -36,15 +35,16 @@ inline int sweep_rows(int m, int64_t R, bool blockn) {
 // warp owns NMBW row blocks (8 basis rows each) x NNB/2 tiles of 8 frequencies x {sin, cos} (the 16 MMA rows), i.e.
 // 4*NNB frequencies; WMW consumer warps split the rows, NWC/WMW split the frequencies of the tile.
 //   CI  TOAs per staged chunk (KB = CI/4 k-blocks)
-//   NWC / NWP  consumer (MMA) / producer (sincos) warps of the CTA. The MMA issue rate of one warp is
-//   limited, so narrow accumulator tiles want three consumer warps per SM sub-partition (12 + 8);
-//   the default is two per sub-partition and four producer warps per sub-partition (8 + 16).
-template <int NMBW_, int NNB_, int WMW_, int CI_, int NWC_ = ffp::NWC, int NWP_ = ffp::NWP>
+//   NWC / NWP  consumer (MMA) / producer (sincos) warps of the CTA. The default is two consumer and four
+//   producer warps per SM sub-partition (8 + 16), where a producer evaluates one sincos chain at a time; the
+//   m <= 80 family runs 8 + 8, whose producers have the registers to evaluate four chains in lockstep.
+//   CREGS / PREGS  setmaxnreg split of the launch-time register pool (NTHREADS x the launch register count)
+template <int NMBW_, int NNB_, int WMW_, int CI_, int NWC_ = ffp::NWC, int NWP_ = ffp::NWP,
+          int CREGS_ = CONSUMER_REGS, int PREGS_ = PRODUCER_REGS>
 struct SweepCfg {
   static constexpr int NMBW = NMBW_, NNB = NNB_, WMW = WMW_, CI = CI_;
   static constexpr int NWC = NWC_, NWP = NWP_, NTC = NWC_ * 32, NTP = NWP_ * 32, NTHREADS = NTC + NTP;
-  // setmaxnreg split of the launch-time register pool (NTHREADS x the launch register count)
-  static constexpr int CREGS = NWC_ == 8 ? CONSUMER_REGS : 112, PREGS = NWC_ == 8 ? PRODUCER_REGS : 64;
+  static constexpr int CREGS = CREGS_, PREGS = PREGS_;
   static_assert(NTHREADS <= 1024 && NWC % WMW_ == 0, "warp layout");
   static_assert(NTC * CREGS + NTP * PREGS <= NTHREADS * ((65536 / NTHREADS) / 8 * 8), "register pool");
   static constexpr int WNW = NWC / WMW;        // consumer warps along frequency
@@ -59,14 +59,22 @@ struct SweepCfg {
   // basis phase: one warp store covers 8 frequencies x 4 TOAs; a thread keeps XW frequencies
   static constexpr int NX = KF / 8;                       // groups of 8 frequencies
   static constexpr int XW = NX >= NWP ? NX / NWP : 1;      // frequency groups per producer warp
-  // producer warps sharing one group split its k-blocks; with few groups and few k-blocks the
-  // surplus warps stay idle (they still take part in the barrier protocol)
-  static constexpr int KSPLIT = NX >= NWP ? 1 : (NWP / NX < KB ? NWP / NX : KB);
-  static constexpr int KBW = KB / KSPLIT;                 // k-blocks per active producer warp
-  static constexpr int NACTIVE = NX >= NWP ? NWP : NX * KSPLIT;  // producer warps with work
+  // the five scalar sums of a group are kept as KSPLIT partial sums over consecutive k-block ranges, added in order
+  // in the epilogue. The partition is the one the default 16 producer warps give (warps sharing a group split its
+  // k-blocks), whatever NWP is, so a frequency's sums are rounded the same way under every producer split.
+  static constexpr int KSPLIT = NX >= ffp::NWP ? 1 : (ffp::NWP / NX < KB ? ffp::NWP / NX : KB);
+  static constexpr int KBW = KB / KSPLIT;                 // k-blocks of one partial sum
+  // producer warps sharing one group, and the partial sums each of them keeps; with few groups and few k-blocks
+  // the surplus warps stay idle (they still take part in the barrier protocol)
+  static constexpr int WPG = NX >= NWP ? 1 : (NWP / NX < KSPLIT ? NWP / NX : KSPLIT);
+  static constexpr int SPW = KSPLIT / WPG;
+  static constexpr int NACTIVE = NX >= NWP ? NWP : NX * WPG;  // producer warps with work
+  // sincos chains a producer thread evaluates in lockstep (sincos_cw_n): lockstep chains need about 72 registers,
+  // so with fewer a thread evaluates one (TOA, frequency) pair at a time
+  static constexpr int NV = PREGS >= 72 ? KBW * XW : 1;
   static constexpr int NACC = 2 * NMBW * NNB;  // accumulators per thread
   static constexpr int NACCX = NACC + 3 * NNB;  // + epoch sums of the block-N variant
-  static constexpr int SLAB = NACCX * NTC + 5 * XW * NTP;  // doubles of level-2 scratch per CTA
+  static constexpr int SLAB = NACCX * NTC + 5 * SPW * XW * NTP;  // doubles of level-2 scratch per CTA
   static constexpr int FLUSH = FLUSH_TOAS / CI;  // chunks per level-1 block
   // ring depths: sin/cos tiles (producer -> consumer) and G tiles (TMA -> consumer), as deep as
   // the shared-memory budget allows
@@ -76,7 +84,8 @@ struct SweepCfg {
   static constexpr int RED = KF * (3 * WMW + 5 * KSPLIT);  // doubles of epilogue reduction scratch
   static constexpr size_t SMEM =
       (size_t)(SST * ST + GST * GT + VST * VEC + KF + RED + 2 * (SST + GST + VST)) * 8 + 128;
-  static_assert(KB % KSPLIT == 0 && NACTIVE <= NWP, "basis-phase mapping");
+  static_assert(KB % KSPLIT == 0 && KSPLIT % WPG == 0 && NACTIVE <= NWP && (KBW * XW) % NV == 0,
+                "basis-phase mapping");
   static_assert(GST >= 3, "the consumers prefetch across chunk boundaries: three G stages at least");
 };
 

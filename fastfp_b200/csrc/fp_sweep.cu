@@ -11,9 +11,11 @@ namespace ffp {
 bool sweep_config(int m, KernelCfg* c) {
   if (m < 1 || m > MAX_M) return false;
   if (m <= 40) { *c = {(m + 7) / 8, 4, 1, 16}; return true; }    // 128 frequencies per CTA
-  // (a 12-consumer/8-producer split with 3 x 4 block warp tiles -- SweepCfg<3, 4, 3, 32, 12, 8> -- was
-  // measured for m = 72: the MMA warps alone get 5% faster, the 8 producer warps fall behind, net -6%)
-  if (m <= 80) { *c = {(m + 7) / 8, 2, 1, 32}; return true; }    // 64 frequencies per CTA
+  // 64 frequencies per CTA on 8 consumer + 8 producer warps (fp_sweep_w2.cu): a producer warp owns a group of 8
+  // frequencies and evaluates its sincos chains four at a time, and the 512-thread register pool leaves the consumers
+  // spill-free. (8 producer warps at one chain each fall behind the MMAs: a 12-consumer/8-producer split measured
+  // -6% net for m = 72.)
+  if (m <= 80) { *c = {(m + 7) / 8, 2, 1, 32}; return true; }
   if (m <= 160) { *c = {(m + 15) / 16, 2, 2, 16}; return true; }  // 32 frequencies per CTA
   if (m <= 320) { *c = {(m + 31) / 32, 2, 4, 16}; return true; }  // 16 frequencies per CTA
   // all eight consumer warps along the rows, chunks of 8 TOAs (the G tile of a chunk is 8 x 640 doubles = 40 KB): 8
@@ -23,7 +25,8 @@ bool sweep_config(int m, KernelCfg* c) {
   return true;
 }
 
-int sweep_max_slab_doubles() { return (40 + 12) * 12 * 32 + 10 * NTP; }  // NACC <= 80, XW <= 2, at most 12 consumer warps
+// NACC <= 80, at most 12 consumer warps; producers keep 5 * SPW * XW <= 10 slots per thread, 512 threads at most
+int sweep_max_slab_doubles() { return (40 + 12) * 12 * 32 + 10 * NTP; }
 
 static int dispatch_group(const fastfp_pack* pk, const GroupView& g, const SweepArgs& a, SweepMode mode,
                           cudaStream_t st) {

@@ -1,6 +1,6 @@
 // The frequency-sweep kernel (fp64 DMMA formulation): a persistent, warp-specialised CTA -- SweepCfg::NWC
-// consumer (MMA) warps + SweepCfg::NWP producer (sincos) warps, 8 + 16 = 768 threads by default, one CTA
-// per SM -- takes (pulsar, frequency-tile) work items from an atomic counter.
+// consumer (MMA) warps + SweepCfg::NWP producer (sincos) warps, 8 + 16 = 768 threads by default and 8 + 8 = 512
+// for m <= 80, one CTA per SM -- takes (pulsar, frequency-tile) work items from an atomic counter.
 //
 // Replaces the body of FastFp.calculate_Fp under jax.vmap (reference fastfp/fastfp.py:69-92,
 // examples/run_fp.py:63) -- and, in SweepMode::Nmfp, the draw-independent part of
@@ -20,10 +20,12 @@
 //                  does at fastfp.py:90); term = 0.5 * N . M^-1 N.
 //
 // Producers and consumers are decoupled by full/empty mbarriers, so the dependent sincos chains of
-// the producers interleave with the consumers' MMAs on the shared fp64 pipe at run time. With the default
-// split each SM sub-partition hosts two consumer warps and four producer warps (the producers' DFMAs queue
-// behind the MMAs on the shared pipe, so it takes that many to keep the S ring full); the register file is
-// split with setmaxnreg (SweepCfg::CREGS / PREGS = 120 / 56 registers per thread out of the 768 x 80 pool).
+// the producers interleave with the consumers' MMAs on the shared fp64 pipe at run time. The producers' DFMAs queue
+// behind the MMAs on the shared pipe, so a sub-partition needs several independent sincos chains in flight to keep
+// the S ring full: with the default split it hosts two consumer warps and four producer warps of one chain each
+// (setmaxnreg split SweepCfg::CREGS / PREGS = 120 / 56 of the 768 x 80 pool); the m <= 80 family hosts two and two,
+// whose producers run four chains in lockstep (168 / 88 of the 512 x 128 pool, which also keeps the consumers'
+// accumulators and fragments out of local memory).
 //
 // The f^(-1/3) prefactor of fastfp.py:78-79 scales N by a and M by a^2 and cancels exactly in
 // N^T M^-1 N; it is not applied (f <= 0 still yields NaN as in the reference).
@@ -103,12 +105,11 @@ struct WorkItem {
 template <class C>
 __device__ __forceinline__ void producer_loop(const SweepArgs& ar, SweepSmem<C>& sm, volatile int* s_work,
                                               const int pw, const int lane) {
-  constexpr int CI = C::CI, XW = C::XW;
+  constexpr int XW = C::XW, SPW = C::SPW, KBW = C::KBW, NV = C::NV;
   const int tidp = pw * 32 + lane;
   const int bk = lane & 3, bf8 = lane >> 2;
-  const int bx0 = C::NX >= C::NWP ? pw * XW : pw % C::NX;         // first group of 8 frequencies
-  const int bkb0 = C::NX >= C::NWP ? 0 : (pw / C::NX) * C::KBW;   // first k-block
-  const int bsplit = C::NX >= C::NWP ? 0 : pw / C::NX;
+  const int bx0 = C::NX >= C::NWP ? pw * XW : pw % C::NX;          // first group of 8 frequencies
+  const int bsplit = C::NX >= C::NWP ? 0 : (pw / C::NX) * SPW;    // first partial sum; its k-blocks from bsplit*KBW
   // element (frequency group x, k-block kb) -> S offset (kb*NX + x)*64 + 2*lane: the (sin, cos) pair of a (TOA,
   // frequency) is the (a0, a1) fragment of the consumer lane with the same (frequency, TOA) -- one 16-byte store,
   // 512 contiguous bytes per warp
@@ -140,11 +141,13 @@ __device__ __forceinline__ void producer_loop(const SweepArgs& ar, SweepSmem<C>&
 #pragma unroll
     for (int xx = 0; xx < XW; ++xx) fast = fast && (fabs(omega[xx]) * pm.tabs_max <= 0.999 * FFP_SINCOS_MAX);
     fast = __all_sync(0xffffffffu, fast);
-    double s2[XW][5];
+    double s2[SPW][XW][5];  // [partial sum][frequency group][sum]
 #pragma unroll
-    for (int xx = 0; xx < XW; ++xx)
+    for (int sp = 0; sp < SPW; ++sp)
 #pragma unroll
-      for (int q = 0; q < 5; ++q) s2[xx][q] = 0.0;
+      for (int xx = 0; xx < XW; ++xx)
+#pragma unroll
+        for (int q = 0; q < 5; ++q) s2[sp][xx][q] = 0.0;
     bool flushed = false;
 
     for (int c = 0; c < nch; ++c) {
@@ -158,51 +161,62 @@ __device__ __forceinline__ void producer_loop(const SweepArgs& ar, SweepSmem<C>&
       const double* pk = sm.Vring + (k % VST) * C::VEC;
       double* sb = sm.Sring + (k % C::SST) * C::ST + sofs;
       if (!FFP_DBG(ar, 1) && pw < C::NACTIVE) {
-        if (fast) {
-          // straight-line: every phase of this tile is inside the Cody-Waite range (checked once per
-          // work item against the pulsar's largest |TOA|), so there is no per-element test
 #pragma unroll
-          for (int kk = 0; kk < C::KBW; ++kk) {
-            const int kb = bkb0 + kk;
-            const int i = 4 * kb + bk;
-            const double2 tn = *reinterpret_cast<const double2*>(pk + 4 * i);  // (t, 1/N)
-            const double wv = pk[4 * i + 2];
+        for (int sp = 0; sp < SPW; ++sp) {
+          // element e of partial sum sp: k-block (bsplit + sp)*KBW + e/XW, frequency group bx0 + e%XW
+          const int kb0 = (bsplit + sp) * KBW;
+          if (fast) {
+            // straight-line: every phase of this tile is inside the Cody-Waite range (checked once per
+            // work item against the pulsar's largest |TOA|), so there is no per-element test; NV elements
+            // at a time, whose sincos chains run in lockstep
 #pragma unroll
-            for (int xx = 0; xx < XW; ++xx) {
-              const double ph = __dmul_rn(omega[xx], tn.x);  // ((2*pi)*f)*t, rounded once more
-              double s, cs;
-              sincos_cw(ph, &s, &cs);
-              *reinterpret_cast<double2*>(sb + (kb * C::NX + bx0 + xx) * 64) = make_double2(s, cs);
-              const double sn = s * tn.y, cn = cs * tn.y;
-              s2[xx][0] = fma(sn, s, s2[xx][0]);
-              s2[xx][1] = fma(sn, cs, s2[xx][1]);
-              s2[xx][2] = fma(cn, cs, s2[xx][2]);
-              s2[xx][3] = fma(s, wv, s2[xx][3]);
-              s2[xx][4] = fma(cs, wv, s2[xx][4]);
-            }
-          }
-        } else {
-          // cold: some phase of this tile may exceed the Cody-Waite range (or is NaN/Inf): library sincos
-#pragma unroll 1
-          for (int e = 0; e < C::KBW * XW; ++e) {
-            const int kb = bkb0 + e / XW, xx = e % XW;
-            const int i = 4 * kb + bk;
-            const double om = __dmul_rn(6.283185307179586, sm.fq[8 * (bx0 + xx) + bf8]);
-            const double ph = __dmul_rn(om, pk[4 * i]);
-            double s, cs;
-            sincos(ph, &s, &cs);
-            const double ni = pk[4 * i + 1], wv = pk[4 * i + 2];
-            *reinterpret_cast<double2*>(sb + (kb * C::NX + bx0 + xx) * 64) = make_double2(s, cs);
-            const double sn = s * ni, cn = cs * ni;
+            for (int e0 = 0; e0 < KBW * XW; e0 += NV) {
+              double ph[NV], s[NV], cs[NV], ni[NV], wv[NV];
 #pragma unroll
-            for (int x2 = 0; x2 < XW; ++x2)
-              if (x2 == xx) {
-                s2[x2][0] = fma(sn, s, s2[x2][0]);
-                s2[x2][1] = fma(sn, cs, s2[x2][1]);
-                s2[x2][2] = fma(cn, cs, s2[x2][2]);
-                s2[x2][3] = fma(s, wv, s2[x2][3]);
-                s2[x2][4] = fma(cs, wv, s2[x2][4]);
+              for (int v = 0; v < NV; ++v) {
+                const int i = 4 * (kb0 + (e0 + v) / XW) + bk;
+                const double2 tn = *reinterpret_cast<const double2*>(pk + 4 * i);  // (t, 1/N)
+                ph[v] = __dmul_rn(omega[(e0 + v) % XW], tn.x);  // ((2*pi)*f)*t, rounded once more
+                ni[v] = tn.y;
+                wv[v] = pk[4 * i + 2];
               }
+              sincos_cw_n<NV>(ph, s, cs);
+#pragma unroll
+              for (int v = 0; v < NV; ++v) {
+                const int kb = kb0 + (e0 + v) / XW, xx = (e0 + v) % XW;
+                *reinterpret_cast<double2*>(sb + (kb * C::NX + bx0 + xx) * 64) = make_double2(s[v], cs[v]);
+                const double sn = s[v] * ni[v], cn = cs[v] * ni[v];
+                double* a = s2[sp][xx];
+                a[0] = fma(sn, s[v], a[0]);
+                a[1] = fma(sn, cs[v], a[1]);
+                a[2] = fma(cn, cs[v], a[2]);
+                a[3] = fma(s[v], wv[v], a[3]);
+                a[4] = fma(cs[v], wv[v], a[4]);
+              }
+            }
+          } else {
+            // cold: some phase of this tile may exceed the Cody-Waite range (or is NaN/Inf): library sincos
+#pragma unroll 1
+            for (int e = 0; e < KBW * XW; ++e) {
+              const int kb = kb0 + e / XW, xx = e % XW;
+              const int i = 4 * kb + bk;
+              const double om = __dmul_rn(6.283185307179586, sm.fq[8 * (bx0 + xx) + bf8]);
+              const double ph = __dmul_rn(om, pk[4 * i]);
+              double s, cs;
+              sincos(ph, &s, &cs);
+              const double ni = pk[4 * i + 1], wv = pk[4 * i + 2];
+              *reinterpret_cast<double2*>(sb + (kb * C::NX + bx0 + xx) * 64) = make_double2(s, cs);
+              const double sn = s * ni, cn = cs * ni;
+#pragma unroll
+              for (int x2 = 0; x2 < XW; ++x2)
+                if (x2 == xx) {
+                  s2[sp][x2][0] = fma(sn, s, s2[sp][x2][0]);
+                  s2[sp][x2][1] = fma(sn, cs, s2[sp][x2][1]);
+                  s2[sp][x2][2] = fma(cn, cs, s2[sp][x2][2]);
+                  s2[sp][x2][3] = fma(s, wv, s2[sp][x2][3]);
+                  s2[sp][x2][4] = fma(cs, wv, s2[sp][x2][4]);
+                }
+            }
           }
         }
       }
@@ -213,14 +227,16 @@ __device__ __forceinline__ void producer_loop(const SweepArgs& ar, SweepSmem<C>&
       }
       if ((c + 1) % C::FLUSH == 0 && c + 1 < nch && !FFP_DBG(ar, 4)) {
 #pragma unroll
-        for (int xx = 0; xx < XW; ++xx)
+        for (int sp = 0; sp < SPW; ++sp)
 #pragma unroll
-          for (int q = 0; q < 5; ++q) {
-            double* a = sl + (size_t)(xx * 5 + q) * C::NTP;
-            if (flushed) atomicAdd(a, s2[xx][q]);  // result unused -> RED.ADD.F64, no round trip
-            else __stcg(a, s2[xx][q]);
-            s2[xx][q] = 0.0;
-          }
+          for (int xx = 0; xx < XW; ++xx)
+#pragma unroll
+            for (int q = 0; q < 5; ++q) {
+              double* a = sl + (size_t)((sp * XW + xx) * 5 + q) * C::NTP;
+              if (flushed) atomicAdd(a, s2[sp][xx][q]);  // result unused -> RED.ADD.F64, no round trip
+              else __stcg(a, s2[sp][xx][q]);
+              s2[sp][xx][q] = 0.0;
+            }
         flushed = true;
       }
     }
@@ -228,22 +244,26 @@ __device__ __forceinline__ void producer_loop(const SweepArgs& ar, SweepSmem<C>&
     // scalar sums: level-2 totals, then across the 4 lanes that share a frequency
     if (flushed) __threadfence();
 #pragma unroll
-    for (int xx = 0; xx < XW; ++xx)
-#pragma unroll
-      for (int q = 0; q < 5; ++q) {
-        double v = s2[xx][q];
-        if (flushed) v += __ldcg(sl + (size_t)(xx * 5 + q) * C::NTP);
-        v += __shfl_xor_sync(0xffffffffu, v, 1);
-        v += __shfl_xor_sync(0xffffffffu, v, 2);
-        s2[xx][q] = v;
-      }
-    double* redA = sm.red + C::WMW * C::KF * 3;  // [KSPLIT][KF][5]
-    if (bk == 0 && pw < C::NACTIVE) {
+    for (int sp = 0; sp < SPW; ++sp)
 #pragma unroll
       for (int xx = 0; xx < XW; ++xx)
 #pragma unroll
-        for (int q = 0; q < 5; ++q)
-          redA[(bsplit * C::KF + 8 * (bx0 + xx) + bf8) * 5 + q] = s2[xx][q];
+        for (int q = 0; q < 5; ++q) {
+          double v = s2[sp][xx][q];
+          if (flushed) v += __ldcg(sl + (size_t)((sp * XW + xx) * 5 + q) * C::NTP);
+          v += __shfl_xor_sync(0xffffffffu, v, 1);
+          v += __shfl_xor_sync(0xffffffffu, v, 2);
+          s2[sp][xx][q] = v;
+        }
+    double* redA = sm.red + C::WMW * C::KF * 3;  // [KSPLIT][KF][5]
+    if (bk == 0 && pw < C::NACTIVE) {
+#pragma unroll
+      for (int sp = 0; sp < SPW; ++sp)
+#pragma unroll
+        for (int xx = 0; xx < XW; ++xx)
+#pragma unroll
+          for (int q = 0; q < 5; ++q)
+            redA[((bsplit + sp) * C::KF + 8 * (bx0 + xx) + bf8) * 5 + q] = s2[sp][xx][q];
     }
     __syncthreads();  // B3: reductions published
     __syncthreads();  // B4: tile finished
@@ -588,11 +608,12 @@ int dispatch_sweep_xwide(const fastfp_pack*, const GroupView&, const SweepArgs&,
 
 // six kernels per configuration: Fp, Nmfp and Res, each with diagonal or block-diagonal N (pk->ecorr; Res: plain-Fp packs
 // only, whose residual packets keep the 8 slot rows last, behind the realisations)
-#define FFP_SWEEP_CASE(NMBWv, NNBv, WMWv, CIv) FFP_SWEEP_CASE_W(NMBWv, NNBv, WMWv, CIv, 8, 16)
-#define FFP_SWEEP_CASE_W(NMBWv, NNBv, WMWv, CIv, NWCv, NWPv)                                       \
+#define FFP_SWEEP_CASE(NMBWv, NNBv, WMWv, CIv) \
+  FFP_SWEEP_CASE_W(NMBWv, NNBv, WMWv, CIv, NWC, NWP, CONSUMER_REGS, PRODUCER_REGS)
+#define FFP_SWEEP_CASE_W(NMBWv, NNBv, WMWv, CIv, NWCv, NWPv, CREGSv, PREGSv)                       \
   if (g.cfg.nmbw == NMBWv && g.cfg.nnb == NNBv && g.cfg.wmw == WMWv && g.cfg.ci == CIv &&          \
       g.cfg.nwc == NWCv) {                                                                         \
-    using Cfg_ = SweepCfg<NMBWv, NNBv, WMWv, CIv, NWCv, NWPv>;                                      \
+    using Cfg_ = SweepCfg<NMBWv, NNBv, WMWv, CIv, NWCv, NWPv, CREGSv, PREGSv>;                      \
     if (mode == SweepMode::Res)                                                                    \
       return pk->ecorr ? launch_sweep_cfg<Cfg_, SweepMode::Res, true>(pk, g, a, st)                \
                        : launch_sweep_cfg<Cfg_, SweepMode::Res, false>(pk, g, a, st);              \

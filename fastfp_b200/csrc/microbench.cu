@@ -329,9 +329,12 @@ __global__ void __launch_bounds__(256, 2) dmma16_peak_kernel(int iters, double s
   if (s == 12345.678) sink[0] = s;
 }
 
-// kind 22: kinds 13-15's warp specialisation with the sweep's m16n8k4 -- 8 warps issue m16n8k4 (8 accumulators each),
-// 16 warps issue DFMA chains, with as many DFMAs per MMA FMA as kind 14 (the sweep kernel's producer ratio)
-__global__ void __launch_bounds__(768, 1) warp_mix16_kernel(int iters, double seed, double* sink) {
+// kinds 22, 25: kinds 13-15's warp specialisation with the sweep's m16n8k4 -- 8 warps issue m16n8k4 (8 accumulators
+// each), NWD warps issue NCH independent DFMA chains each, with as many DFMAs per MMA FMA as kind 14 (the sweep kernel's
+// producer ratio). Kind 22: 16 warps x 16 chains (768 threads); kind 25: 8 warps x 4 chains (512 threads, the m <= 80
+// sweep's split, whose producers run four sincos chains in lockstep).
+template <int NWD, int NCH>
+__global__ void __launch_bounds__(32 * (8 + NWD), 1) warp_mix16_kernel(int iters, double seed, double* sink) {
   const int w = threadIdx.x >> 5;
   double s = 0;
   if (w < 8) {
@@ -346,18 +349,19 @@ __global__ void __launch_bounds__(768, 1) warp_mix16_kernel(int iters, double se
 #pragma unroll
     for (int k = 0; k < 8; ++k) s += c[k][0] + c[k][1] + c[k][2] + c[k][3];
   } else {
-    // twice kind 14's DFMA iterations: a DMMA warp iteration here is 8 x 512 FMAs, there 8 x 256
-    const int itf = (int)((long long)iters * 4 * 50 / 256);
-    double a[16];
+    // twice kind 14's DFMA iterations: a DMMA warp iteration here is 8 x 512 FMAs, there 8 x 256; the same DFMAs per
+    // SM whatever NWD x NCH
+    const int itf = (int)((long long)iters * 4 * 50 / 256) * (16 * 16 / (NWD * NCH));
+    double a[NCH];
 #pragma unroll
-    for (int k = 0; k < 16; ++k) a[k] = seed + k + threadIdx.x * 1e-3;
+    for (int k = 0; k < NCH; ++k) a[k] = seed + k + threadIdx.x * 1e-3;
     const double x = 1.0000001, y = 1e-9;
     for (int it = 0; it < itf; ++it) {
 #pragma unroll
-      for (int k = 0; k < 16; ++k) a[k] = fma(a[k], x, y);
+      for (int k = 0; k < NCH; ++k) a[k] = fma(a[k], x, y);
     }
 #pragma unroll
-    for (int k = 0; k < 16; ++k) s += a[k];
+    for (int k = 0; k < NCH; ++k) s += a[k];
   }
   if (s == 12345.678) sink[0] = s;
 }
@@ -440,7 +444,8 @@ int run_fp64_peak(int kind, int iters, double* tflops, double* ms_out) {
     else if (kind == 1) dmma16_peak_kernel<4><<<sms * 2, 256>>>(iters, 1.0, sink);    // 4 warps / sub-partition
     else if (kind == 20) dmma16_peak_kernel<8><<<sms * 2, 256>>>(iters, 1.0, sink);
     else if (kind == 21) dmma16_peak_kernel<16><<<sms * 2, 256>>>(iters, 1.0, sink);
-    else if (kind == 22) warp_mix16_kernel<<<sms, 768>>>(iters, 1.0, sink);
+    else if (kind == 22) warp_mix16_kernel<16, 16><<<sms, 768>>>(iters, 1.0, sink);
+    else if (kind == 25) warp_mix16_kernel<8, 4><<<sms, 512>>>(iters, 1.0, sink);
     else if (kind == 23) dmma16_tile_kernel<9, 4><<<sms, 256>>>(iters, 1.0, sink);     // 2 warps / sub-partition
     else if (kind == 24) dmma16_tile_kernel<9, 8><<<sms, 256>>>(iters, 1.0, sink);
     else if (kind == 2) mixed_peak_kernel<<<grid, 256>>>(iters, 1.0, sink);
@@ -467,7 +472,7 @@ int run_fp64_peak(int kind, int iters, double* tflops, double* ms_out) {
                            : kind == 19 ? (double)grid * 8 * 8.0 * 256.0 * iters
                            : kind == 1 || kind == 20 || kind == 21
                                ? (double)sms * 16 * 8 * (128.0 * (kind == 1 ? 4 : kind == 20 ? 8 : 16)) * iters
-                           : kind == 22 ? (double)sms * (8 * 8 * 512.0 * iters +
+                           : kind == 22 || kind == 25 ? (double)sms * (8 * 8 * 512.0 * iters +
                                                          16 * 32 * 16.0 * (double)((long long)iters * 4 * 50 / 256))
                            : kind == 23 || kind == 24 ? (double)sms * 8 * 2 * 9 * (128.0 * (kind == 23 ? 4 : 8)) * iters
                            : kind == 9 ? (double)sms * 8 * 2 * 18 * 256.0 * iters

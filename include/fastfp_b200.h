@@ -362,7 +362,8 @@ int fastfp_xcy_blockn(int device, int64_t n, int64_t m, const double* Nvec, cons
  * are the kernel-design probes of csrc/microbench.cu; 13-15 run the sweep kernel's warp
  * specialisation (8 DMMA warps + 16 DFMA warps) on registers only; 16 = legacy INT8 mma.sync rate
  * (reported as 2 x MAC/s in the same unit); 17 = s8 wgmma m64n256k32 on two warpgroups (the INT8 tensor peak, TOP/s);
- * 18 = the tensor sweep's own stage (28 plane products, two warpgroups of m64n32k32). */
+ * 18 = the tensor sweep's own stage (28 plane products, two warpgroups of m64n32k32); 19-24 the fp64 MMA shapes and
+ * consumer tiles; 22 / 25 the warp specialisation on m16n8k4 at the 8 + 16 and 8 + 8 warp splits. */
 int fastfp_fp64_peak(int device, int kind, int iters, double* tflops, double* ms);
 
 #ifdef __cplusplus
