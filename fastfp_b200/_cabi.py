@@ -114,10 +114,22 @@ SYMBOLS = {
          C.c_void_p, C.c_void_p],
     ),
     "fastfp_fp64_peak": (C.c_int, [C.c_int, C.c_int, C.c_int, c_double_p, c_double_p]),
+    "fastfp_row_groups": (C.c_int, [C.c_int64, C.POINTER(C.c_int64)]),
 }
 
 
 MAX_M = 640  # G rows of the widest sweep kernel (csrc/ffp_internal.cuh)
+MAX_M_WIDE = 2688  # widest basis of a diagonal-N Fp pack, swept as row groups of at most MAX_M rows (DESIGN.md 5h)
+
+
+def row_groups(m: int):
+    """The row groups the library sweeps a basis of width ``m`` in (``fastfp_row_groups``): a list of ``(start, stop)``
+    row ranges, one for ``m <= MAX_M``. Raises ``ValueError`` outside ``1 .. MAX_M_WIDE``."""
+    starts = (C.c_int64 * (m // 8 + 2))() if 1 <= m <= MAX_M_WIDE else None
+    g = load().fastfp_row_groups(int(m), starts)
+    if g < 1:
+        raise ValueError(f"basis width m={m} is outside 1 .. {MAX_M_WIDE}")
+    return [(starts[k], starts[k + 1]) for k in range(g)]
 
 
 def sweep_rows(m: int, R: int = 0, blockn: bool = False) -> int:
@@ -129,7 +141,11 @@ def sweep_rows(m: int, R: int = 0, blockn: bool = False) -> int:
 def max_residual_rows(m, blockn: bool = False) -> int:
     """Most residual realisations ``fastfp_pack_set_residuals`` takes for pulsars of basis widths ``m``: every pulsar
     needs :func:`sweep_rows` of the sweep kernel's ``MAX_M`` G rows. A block-diagonal N pack
-    (``fastfp_pack_set_residuals_blockn``) needs 8 more, the epoch slots."""
+    (``fastfp_pack_set_residuals_blockn``) needs 8 more, the epoch slots. Residual batches take no basis wider than
+    ``MAX_M`` columns (row groups are for plain sweeps): ``ValueError`` for such a pulsar."""
+    if max(m) > MAX_M:
+        raise ValueError(f"residual batches need every basis to be at most {MAX_M} columns wide; pulsar "
+                         f"{list(m).index(max(m))} has a basis wider than {MAX_M} (m = {max(m)})")
     return MAX_M - sweep_rows(max(m), 0, blockn)
 
 
@@ -327,6 +343,11 @@ class Pack:
             what = "sigmas" if m_fix is None else "TNTs"
             P, n, m, toas, residuals, Nvecs, Ts, mats = _check_lists(toas, residuals, Nvecs, Ts, mats, what)
         nmfp, fixed = m_fix is not None, (None, None)
+        top = MAX_M if nmfp else MAX_M_WIDE  # block-N widths are checked above
+        for p, mp_ in enumerate(m):
+            if not block and mp_ > top:
+                raise ValueError(f"pulsar {p}: basis width {mp_} exceeds the maximum {top} of "
+                                 + ("a noise-marginalised pack" if nmfp else "a diagonal-N pack"))
         if nmfp:
             if len(m_fix) != P or len(phiinv_fix) != P:
                 raise ValueError("m_fix and phiinv_fix must have one entry per pulsar")

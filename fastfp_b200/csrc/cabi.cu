@@ -60,11 +60,14 @@ static int pack_layout(fastfp_pack* pk, int P, const int64_t* n, const int64_t* 
     }
     PulsarMeta& pm = pk->meta[p];
     pm.n = (int)n[p];
-    if (m[p] > MAX_M || !lay.place(p, sweep_rows((int)m[p], 0, blockn), &pm)) {
+    // bases wider than one work item: row groups, placed after the loop (diagonal-N Fp packs only)
+    const bool grouped = !blockn && !m_fix && m[p] > MAX_M && m[p] <= MAX_M_WIDE;
+    if (!grouped && (m[p] > MAX_M || !lay.place(p, sweep_rows((int)m[p], 0, blockn), &pm))) {
       set_error("pulsar " + std::to_string(p) + ": basis width m=" + std::to_string(m[p]) +
                 (blockn ? " exceeds the block-N maximum " + std::to_string(MAX_M - 8) + " (the widest kernel has " +
                               std::to_string(MAX_M) + " rows, 8 of them hold the epoch slots)"
-                        : " exceeds the supported maximum " + std::to_string(MAX_M)));
+                 : m_fix ? " exceeds the noise-marginalised maximum " + std::to_string(MAX_M)
+                         : " exceeds the supported maximum " + std::to_string(MAX_M_WIDE)));
       return FASTFP_ERR_UNSUPPORTED;
     }
     pm.m = (int)m[p];
@@ -98,9 +101,34 @@ static int pack_layout(fastfp_pack* pk, int P, const int64_t* n, const int64_t* 
     T_off += (int64_t)pm.n * pm.m;
   }
   pk->mvar_total = var_off;
+  // row groups (DESIGN.md section 5h): one work item per group, meta indices P ..., each placed like a pulsar of its
+  // rows: group 0 of every wide pulsar first, then the other groups pulsar by pulsar
+  std::vector<int> wide;
+  for (int p = 0; p < P; ++p)
+    if (row_groups(pk->meta[p].m) > 1) wide.insert(wide.end(), {p, 0, 0, row_groups(pk->meta[p].m)});
+  for (int pass = 0; pass < 2; ++pass)
+    for (size_t w = 0; w < wide.size(); w += RG_WIDE) {
+      const PulsarMeta& pm = pk->meta[wide[w]];
+      wide[w + 1 + pass] = P + (int)pk->items.size();
+      for (int k = pass; k < (pass ? wide[w + 3] : 1); ++k) {
+        PulsarMeta it = pm;
+        it.m = it.mfix = row_group_start(pm.m, k + 1) - row_group_start(pm.m, k);
+        it.mvar = 0;
+        lay.place(P + (int)pk->items.size(), sweep_rows(it.m, 0, false), &it);  // <= 288 rows: always placed
+        pk->items.push_back(it);
+      }
+    }
+  pk->n_wide = (int)wide.size() / RG_WIDE;
+  const int nmeta = P + (int)pk->items.size();
   PackCore& c = pk->core;
-  FFP_CUDA(dev_alloc(&c.meta, (size_t)P));
+  FFP_CUDA(dev_alloc(&c.meta, (size_t)nmeta));
   FFP_CUDA(cudaMemcpy(c.meta.get(), pk->meta.data(), sizeof(PulsarMeta) * P, cudaMemcpyHostToDevice));
+  if (pk->n_wide) {
+    FFP_CUDA(cudaMemcpy(c.meta.get() + P, pk->items.data(), sizeof(PulsarMeta) * pk->items.size(),
+                        cudaMemcpyHostToDevice));
+    FFP_CUDA(dev_alloc(&c.wide, wide.size()));
+    FFP_CUDA(cudaMemcpy(c.wide.get(), wide.data(), sizeof(int) * wide.size(), cudaMemcpyHostToDevice));
+  }
   FFP_CUDA(dev_alloc(&c.packets, (size_t)lay.size));
   FFP_CUDA(dev_alloc(&c.L, (size_t)L_off));
   FFP_CUDA(dev_alloc(&c.info, (size_t)P));
@@ -109,7 +137,8 @@ static int pack_layout(fastfp_pack* pk, int P, const int64_t* n, const int64_t* 
   const size_t slab_doubles = (size_t)CTAS_PER_SM * pk->num_sms * sweep_max_slab_doubles();
   FFP_CUDA(dev_alloc(&c.slab, slab_doubles));
   FFP_CUDA(dev_alloc(&c.counter, 1));
-  pk->bytes = lay.size * 8 + L_off * 8 + (int64_t)sizeof(PulsarMeta) * P + (int64_t)slab_doubles * 8;
+  pk->bytes = lay.size * 8 + L_off * 8 + (int64_t)sizeof(PulsarMeta) * nmeta + (int64_t)slab_doubles * 8 +
+              (int64_t)sizeof(int) * wide.size();
   return lay.upload(&pk->groups);
 }
 
@@ -302,6 +331,13 @@ struct ScratchLayout {
 // The limit of a residual batch: every pulsar takes sweep_rows(m, R, blockn) of the kernel's MAX_M G rows, so the widest
 // one bounds R. FASTFP_ERR_UNSUPPORTED with a message that names the limit and that pulsar for an R above it.
 static int check_res_limit(const fastfp_pack* pk, int64_t R, const char* fn) {
+  for (int p = 0; p < pk->P && R > 0; ++p)  // R == 0 releases a set, which any pack may do
+    if (pk->meta[p].m > MAX_M) {
+      set_error(std::string(fn) + ": pulsar " + std::to_string(p) + " has a basis wider than " + std::to_string(MAX_M) +
+                " columns (m = " + std::to_string(pk->meta[p].m) + "); residual batches take bases up to " +
+                std::to_string(MAX_M) + " columns");
+      return FASTFP_ERR_UNSUPPORTED;
+    }
   int wide = 0;
   for (int p = 0; p < pk->P; ++p)
     if (pk->meta[p].m > pk->meta[wide].m) wide = p;
@@ -416,6 +452,13 @@ int fastfp_sweep_chunk_toas(int64_t m, int blockn) {
   return kc.ci;
 }
 
+int fastfp_row_groups(int64_t m, int64_t* starts) {
+  if (m < 1 || m > MAX_M_WIDE) return 0;
+  const int g = row_groups((int)m);
+  for (int k = 0; starts && k <= g; ++k) starts[k] = row_group_start((int)m, k);
+  return g;
+}
+
 int fastfp_pack_create_blockn(int device, int P, const int64_t* n, const int64_t* m,
                               const double* const* toas, const double* const* residuals,
                               const double* const* residuals_w, const double* const* Nvecs,
@@ -433,7 +476,9 @@ int fastfp_pack_create_blockn(int device, int P, const int64_t* n, const int64_t
 }
 
 void fastfp_pack_destroy(fastfp_pack_t* pack) { pack_free(pack); }
-int64_t fastfp_pack_bytes(const fastfp_pack_t* pack) { return pack ? pack->bytes + pack->res.bytes : 0; }
+int64_t fastfp_pack_bytes(const fastfp_pack_t* pack) {
+  return pack ? pack->bytes + pack->res.bytes + pack->rg.cap * 8 : 0;
+}
 int fastfp_pack_num_pulsars(const fastfp_pack_t* pack) { return pack ? pack->P : 0; }
 int64_t fastfp_pack_mvar_total(const fastfp_pack_t* pack) { return pack ? pack->mvar_total : 0; }
 int fastfp_pack_factor_info(const fastfp_pack_t* pack, int32_t* info) {
@@ -457,19 +502,27 @@ static int fp_run(const fastfp_pack* pk, const double* freqs, int64_t F, double*
   if (F == 0) return FASTFP_OK;
   const int P = pk->P;
   const int64_t nout = want_terms ? (int64_t)P * F : F;
+  // the batches bound the terms scratch and, with wide pulsars, the row-group scratch; the terms of a call go straight
+  // to its output unless a pack with wide pulsars needs more than one batch for them
+  const int64_t FB = freq_batch(F, P + pk->rg_doubles_per_freq());
+  const bool direct = want_terms && (FB >= F || !pk->n_wide);
   PackCall c(pk, stream);
   const double* d_freqs;
   double* d_out;
-  if (int rc = c.stage(freqs, F, out, nout, flags, &d_freqs, &d_out, want_terms ? &pk->terms : &pk->out)) return rc;
-  if (want_terms) {
+  if (int rc = c.stage(freqs, F, out, nout, flags, &d_freqs, &d_out, direct ? &pk->terms : &pk->out)) return rc;
+  if (direct) {
     if (int rc = launch_sweep(pk, d_freqs, F, FpOut{d_out, nullptr}, c.st)) return rc;
   } else {
-    const int64_t FB = freq_batch(F, P);
     if (int rc = pk->terms.grow((int64_t)P * std::min(FB, F))) return rc;
     for (int64_t lo = 0; lo < F; lo += FB) {
       const int64_t fb = std::min(FB, F - lo);
       if (int rc = launch_sweep(pk, d_freqs + lo, fb, FpOut{pk->terms.get(), nullptr}, c.st)) return rc;
-      if (int rc = launch_reduce_terms_rows(pk->terms.get(), 1, P, fb, d_out + lo, F, c.st)) return rc;
+      if (want_terms) {
+        FFP_CUDA(cudaMemcpy2DAsync(d_out + lo, (size_t)F * 8, pk->terms.get(), (size_t)fb * 8, (size_t)fb * 8,
+                                   (size_t)P, cudaMemcpyDeviceToDevice, c.st));
+      } else if (int rc = launch_reduce_terms_rows(pk->terms.get(), 1, P, fb, d_out + lo, F, c.st)) {
+        return rc;
+      }
     }
   }
   return c.finish(flags, nout, out, d_out, false);
@@ -654,7 +707,7 @@ int fastfp_fe_sweep(const fastfp_pack_t* pk, const double* freqs, int64_t F, con
   const double* d_freqs;
   double* d_out;
   if (int rc = c.stage(freqs, F, out, S * F, flags, &d_freqs, &d_out, &pk->out)) return rc;
-  const int64_t FB = freq_batch(F, 5 * (int64_t)P);
+  const int64_t FB = freq_batch(F, 5 * (int64_t)P + pk->rg_doubles_per_freq());
   // scratch: the inner products of one frequency batch, then the antenna patterns of the S sky positions
   ScratchLayout lay;
   const int64_t o_inner = lay.take(5 * (int64_t)P * std::min(FB, F)), o_fp = lay.take(S * P), o_fx = lay.take(S * P);
@@ -685,7 +738,7 @@ int fastfp_fe_skymax(const fastfp_pack_t* pk, const double* freqs, int64_t F, co
   const double* d_freqs;
   double* d_max;
   if (int rc = c.stage(freqs, F, fe_max, F, flags, &d_freqs, &d_max, &pk->out)) return rc;
-  const int64_t FB = freq_batch(F, 5 * (int64_t)P);
+  const int64_t FB = freq_batch(F, 5 * (int64_t)P + pk->rg_doubles_per_freq());
   const int64_t fb0 = std::min(FB, F);
   const FeSkyPlan plan = fe_skymax_plan(fb0, S, pk->num_sms);
   // scratch, all in the pack's Fe buffer: the inner products of one frequency batch, the antenna patterns and the

@@ -24,6 +24,23 @@ constexpr int CONSUMER_REGS = 120, PRODUCER_REGS = 56;  // default setmaxnreg sp
 constexpr int VST = 16;        // TOA-vector ring depth (t | 1/N | w; TMA -> producer)
 constexpr int FLUSH_TOAS = 512;  // level-1 accumulation block, in TOAs
 constexpr int MAX_M = 640;     // widest basis the sweep kernel handles (8 warp rows x 10 blocks of 8 rows)
+// Wider bases (diagonal-N Fp packs only, DESIGN.md section 5h) are swept as row groups of G, each one work item of the
+// kernel: ceil(m / RG_ROWS) groups of near-equal width in whole blocks of 8 rows, up to MAX_M_WIDE columns. Groups of at
+// most 288 rows run on the 16-frequency family with at most 9 row blocks per warp, measured at 0.57-0.59 ns per
+// (frequency, pulsar, G row) on an H100, against 1.06 at 10 blocks (320 rows) and 0.90-0.94 on the 8-frequency family
+// (DESIGN.md section 5h)
+constexpr int RG_ROWS = 288;
+constexpr int MAX_M_WIDE = 2688;  // 10 groups of 264-272 rows
+constexpr int MAX_RG = (MAX_M_WIDE + RG_ROWS - 1) / RG_ROWS;
+
+// the row groups of a basis of width m (1: the whole basis is one work item) and the first row of group k (k == groups:
+// m); the one statement of the split rule
+__host__ __device__ inline int row_groups(int m) { return m <= MAX_M ? 1 : (m + RG_ROWS - 1) / RG_ROWS; }
+__host__ __device__ inline int row_group_start(int m, int k) {
+  const int nb = (m + 7) / 8, g = row_groups(m);
+  const int r = 8 * (k * (nb / g) + (k < nb % g ? k : nb % g));
+  return r < m ? r : m;
+}
 
 // G rows a pulsar of basis width m takes in the sweep kernel: its basis rows, then R residual realisations from row
 // roundup8(m) on (residual batches, DESIGN.md section 5d), then with a block-diagonal N the 8 epoch-slot rows last
@@ -113,6 +130,12 @@ struct PulsarMeta {
   int32_t i8_nst;      // tensor path: stages of 32 TOAs
   double ninv_sum;     // tensor path: sum_i 1/N_i (c N^-1 c = sum 1/N - s N^-1 s, so the producers form two sums, not three)
 };
+// Row groups (DESIGN.md section 5h): the device meta holds the P pulsars, then one work item per row group of each wide
+// pulsar, each with the pulsar's entry except its own ci, nch, mpad, pk_off and m = mfix = its row count -- first group 0
+// of every wide pulsar, in pulsar order, then the other groups, pulsar by pulsar in group order. A wide pulsar's own
+// entry describes the whole basis and is not swept. PackCore::wide lists per wide pulsar RG_WIDE ints: the pulsar, the
+// meta index of its group 0, that of its group 1 (groups 2 ... follow it) and its number of groups.
+constexpr int RG_WIDE = 4;
 
 struct KernelCfg {  // run-time mirror of SweepCfg's parameters
   int nmbw, nnb, wmw, ci;
@@ -230,7 +253,8 @@ struct Scratch {
 
 // every pack (pack_layout; the slot masks: block-N packs, stage_slots)
 struct PackCore {
-  DeviceBuf<PulsarMeta> meta;
+  DeviceBuf<PulsarMeta> meta;          // [P + row-group items]
+  DeviceBuf<int> wide;                 // [RG_WIDE x wide pulsars] (row groups, see PulsarMeta)
   DeviceBuf<double> packets;           // [sum_p nch_p][PK_p]
   DeviceBuf<double> L;                 // Cholesky factors (Fp) / fixed-block factors (nmfp)
   DeviceBuf<int> info;                 // per-pulsar factorisation status
@@ -289,6 +313,8 @@ struct fastfp_pack {
   bool nmfp = false;
   bool ecorr = false;            // block-diagonal N (kernel ECORR): 8 epoch-slot rows in the G tiles
   std::vector<ffp::PulsarMeta> meta;
+  std::vector<ffp::PulsarMeta> items;  // the row-group work items, meta indices P ... (DESIGN.md section 5h)
+  int n_wide = 0;                       // pulsars with row groups
   std::vector<ffp::Group> groups;
   std::vector<int> info;         // host copy of core.info, read back when the pack is built (fastfp_pack_factor_info)
   ffp::PackCore core;
@@ -310,6 +336,9 @@ struct fastfp_pack {
   mutable ffp::Scratch<double> scratch;  // nmfp: stage-A tiles of a frequency batch
   mutable ffp::Scratch<double> lf;       // nmfp: L^-1 fragments of a draw batch
   mutable ffp::Scratch<double> inner;    // Fe-statistic: inner products of a frequency batch + antenna patterns
+  mutable ffp::Scratch<double> rg;       // row groups: the partial sums of a frequency batch (RowGroupOut)
+  // doubles of row-group scratch per frequency of a sweep (0 without wide pulsars): callers size their batches with it
+  int64_t rg_doubles_per_freq() const { return 5 * (int64_t)n_wide + 3 * ((int64_t)items.size() - n_wide); }
   mutable ffp::PowerlawStaging pl;
   ffp::ResidualBatch res;
   // optional per-stage timing of nmfp sweeps (fastfp_nmfp_stage_timing): stage A, factor, stage B
@@ -555,6 +584,30 @@ struct FpOut {
   }
 };
 
+// plain Fp / Fe of wide pulsars (DESIGN.md section 5h): what their row-group items write, for row_group_combine_kernel.
+// Group 0 of wide pulsar w (meta index first + w) writes (s|s) - b_0, (s|c) - b_0, (c|c) - b_0, (s|r), (c|r) through
+// FpOut::put into part [nwide][F][5] at row w; every other item (meta index first + nwide + k) writes its raw b-sums
+// b_ss, b_sc, b_cc into b [items - nwide][F][3] at row k. Meta indices below first are whole pulsars.
+struct RowGroupOut {
+  double* part;
+  double* b;
+  int first;  // P
+  int nwide;
+  __device__ __forceinline__ double* part_at(int w, int64_t f, int64_t F) const { return part + ((size_t)w * F + f) * 5; }
+  __device__ __forceinline__ double* b_at(int k, int64_t f, int64_t F) const { return b + ((size_t)k * F + f) * 3; }
+  // item `item`, frequency f: producer sums a = (sNs, sNc, cNc, s.w, c.w), b-sums of its rows bs
+  __device__ __forceinline__ void put(int item, int64_t f, int64_t F, const double& fq, const double (&a)[5],
+                                      const double (&bs)[3]) const {
+    const int k = item - first;
+    if (k < nwide) {
+      FpOut{nullptr, part}.put(k, f, F, fq, a[0] - bs[0], a[1] - bs[1], a[2] - bs[2], a[3], a[4]);
+    } else {
+      double* o = b_at(k - nwide, f, F);
+      o[0] = bs[0]; o[1] = bs[1]; o[2] = bs[2];
+    }
+  }
+};
+
 // nmfp stage A, per 32-frequency tile: z'_s, z'_c of the per-draw rows,
 // Z [P][nt32][mvpad/4][8][32], and the draw-independent a-terms a_ss, a_sc, a_cc (fixed block removed), a_sr, a_cr,
 // A [P][nt32][5][32]
@@ -608,6 +661,8 @@ struct ResOut {
 };
 
 // ---- sweep launchers (fp_sweep*.cu), each with the output block of its mode ----------------
+// with wide pulsars, also their row-group combine into `out`, through the pack's row-group scratch
+// (pk->rg_doubles_per_freq() doubles per frequency)
 int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, const FpOut& out, cudaStream_t st,
                     bool rest_only = false);
 int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, const NmfpTiles& out, cudaStream_t st,

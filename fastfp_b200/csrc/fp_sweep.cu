@@ -64,11 +64,43 @@ static int launch_fp_groups(const fastfp_pack* pk, SweepArgs a, SweepMode mode, 
   return 0;
 }
 
+// Row groups (DESIGN.md section 5h): per (wide pulsar, frequency), M = ((sNs - b_0) - b_1) - ... in group order for
+// ss, sc and cc, then the term and the inner products exactly as FpOut::put writes those of a whole pulsar
+__global__ void row_group_combine_kernel(const int* __restrict__ wide, const double* __restrict__ freqs, int64_t F,
+                                         const FpOut out, const RowGroupOut rg) {
+  const int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= F) return;
+  const int* wl = wide + RG_WIDE * blockIdx.y;
+  const int p = wl[0], k1 = wl[2] - rg.first - rg.nwide, g = wl[3];
+  const double* a = rg.part_at(blockIdx.y, f, F);
+  double ss = a[0], sc = a[1], cc = a[2];
+  for (int k = 1; k < g; ++k) {
+    const double* b = rg.b_at(k1 + k - 1, f, F);
+    ss -= b[0];
+    sc -= b[1];
+    cc -= b[2];
+  }
+  const double fq = freqs[f];
+  out.put(p, f, F, fq, ss, sc, cc, a[3], a[4]);
+}
+
 int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, const FpOut& out, cudaStream_t st,
                     bool rest_only) {
   SweepArgs a = sweep_args(pk->core.packets.get(), pk->core.meta.get(), pk, d_freqs, F);
   a.fp = out;
-  return launch_fp_groups(pk, a, SweepMode::Fp, rest_only, st);
+  a.rg = RowGroupOut{nullptr, nullptr, pk->P, pk->n_wide};  // meta indices >= P are row-group items
+  if (pk->n_wide) {
+    if (int rc = pk->rg.grow(pk->rg_doubles_per_freq() * F)) return rc;
+    a.rg.part = pk->rg.get();
+    a.rg.b = pk->rg.get() + 5 * (int64_t)pk->n_wide * F;
+  }
+  if (int rc = launch_fp_groups(pk, a, SweepMode::Fp, rest_only, st)) return rc;
+  if (!pk->n_wide) return 0;
+  row_group_combine_kernel<<<dim3((unsigned)((F + 255) / 256), (unsigned)pk->n_wide), 256, 0, st>>>(
+      pk->core.wide.get(), d_freqs, F, out, a.rg);
+  g_launches += 1;
+  FFP_CUDA(cudaGetLastError());
+  return 0;
 }
 
 int launch_fp_sweep(const fastfp_pack* pk, const double* d_freqs, int64_t F, const NmfpTiles& out, cudaStream_t st,

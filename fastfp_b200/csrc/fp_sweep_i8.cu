@@ -751,7 +751,7 @@ int build_i8_planes(fastfp_pack* pk, cudaStream_t st) {
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   if (e != cudaSuccess) return cuda_fail(e, "build_i8_planes");
   // pulsars with a non-finite G or w (singular Sigma, NaN data) cannot be carried by integer planes: fp64 kernel
-  std::vector<int> take, rest_flag(P, 1);
+  std::vector<int> take, rest_flag(P + pk->items.size(), 1);  // row-group items (wide pulsars) stay on the fp64 kernel
   for (int p = 0; p < P; ++p) {
     const bool ok = pk->meta[p].i8_nst > 0 && bad[p] == 0 && (p >= (int)pk->info.size() || pk->info[p] == 0);
     if (ok) { take.push_back(p); rest_flag[p] = 0; }

@@ -58,6 +58,7 @@ struct SweepArgs {
     NmfpTiles nm;
     ResOut res;
   };
+  RowGroupOut rg;         // SweepMode::Fp: the outputs of row-group items (DESIGN.md section 5h)
   double* slab;           // level-2 scratch, SLAB doubles per CTA
   unsigned int* counter;  // work counter (zeroed before the launch)
   const unsigned char* done_mask;  // block-N packs: per chunk, which of the 8 epoch slots end there
@@ -537,7 +538,10 @@ __device__ __forceinline__ void consumer_loop(const SweepArgs& ar, SweepSmem<C>&
       for (int g2 = 0; g2 < C::KSPLIT; ++g2)
 #pragma unroll
         for (int k = 0; k < 5; ++k) a[k] += redA[(g2 * C::KF + tid) * 5 + k];
-      if (MODE == SweepMode::Fp) ar.fp.put(p, fidx, ar.F, sm.fq[tid], a[0] - b[0], a[1] - b[1], a[2] - b[2], a[3], a[4]);
+      if (MODE == SweepMode::Fp) {
+        if (p < ar.rg.first) ar.fp.put(p, fidx, ar.F, sm.fq[tid], a[0] - b[0], a[1] - b[1], a[2] - b[2], a[3], a[4]);
+        else ar.rg.put(p, fidx, ar.F, sm.fq[tid], a, b);
+      }
       if (MODE == SweepMode::Nmfp) ar.nm.put_a(p, fidx, (ar.F + 31) >> 5, a[0] - b[0], a[1] - b[1], a[2] - b[2], a[3], a[4]);
       if (MODE == SweepMode::Res) {
         // M of this frequency for every realisation; slot 0 of redB for this frequency is read by this thread only

@@ -26,6 +26,7 @@ __global__ void chol_kernel(double* __restrict__ Lbuf, const PulsarMeta* __restr
                             int* __restrict__ info) {
   const PulsarMeta pm = meta[blockIdx.x];
   const int m = pm.m;
+  if (row_groups(m) > 1) return;  // wide pulsars: the blocked factorisation below
   double* A = Lbuf + pm.L_off;
   __shared__ double djj;
   for (int j = 0; j < pm.mfix; ++j) {
@@ -53,8 +54,151 @@ __global__ void chol_kernel(double* __restrict__ Lbuf, const PulsarMeta* __restr
   }
 }
 
-// One thread per (padded) TOA: forward-substitute L g = T_i^T / N_i and scatter t, 1/N and g
-// into the packet layout. Padded TOAs get zeros (weight 0: they add nothing to any sum).
+// The meta of row group k of pulsar p, a wide one (PackCore::wide, n_wide entries)
+__device__ inline const PulsarMeta& group_meta(const PulsarMeta* meta, const int* wide, int n_wide, int p, int k) {
+  int w = 0;
+  while (wide[RG_WIDE * w] != p) ++w;
+  return meta[k == 0 ? wide[RG_WIDE * w + 1] : wide[RG_WIDE * w + 2] + k - 1];
+}
+
+// ---- blocked Cholesky of the wide pulsars (row groups, DESIGN.md section 5h) -------------------------------------
+// Panels of CB columns, left to right: chol_diag_kernel factors the diagonal block in shared memory, chol_panel_kernel
+// solves the rows below it against that block, chol_update_kernel subtracts the panel's outer product from the
+// trailing lower triangle, tile by tile over many CTAs. Every element receives exactly the operations of chol_kernel in
+// the same order -- one fma per earlier column, ascending, then the division by its pivot's square root -- so the factor
+// is bit for bit the unblocked one; only the work is spread over the GPU. One launch of each per panel covers every wide
+// pulsar (PackCore::wide); a pulsar whose basis ends before the panel returns at once.
+constexpr int CB = 32;
+
+__global__ void chol_diag_kernel(double* __restrict__ Lbuf, const PulsarMeta* __restrict__ meta, int* __restrict__ info,
+                                 const int* __restrict__ wide, int k0) {
+  const int p = wide[RG_WIDE * blockIdx.x];
+  const PulsarMeta pm = meta[p];
+  const int m = pm.m;
+  if (k0 >= m) return;
+  const int nb = m - k0 < CB ? m - k0 : CB;
+  double* A = Lbuf + pm.L_off;
+  __shared__ double s[CB][CB + 1];
+  __shared__ double djj;
+  for (int idx = threadIdx.x; idx < nb * nb; idx += blockDim.x) {
+    const int r = idx / nb, c = idx - r * nb;
+    if (c <= r) s[r][c] = A[(size_t)(k0 + r) * m + k0 + c];
+  }
+  __syncthreads();
+  for (int j = 0; j < nb; ++j) {
+    if (threadIdx.x == 0) {
+      const double d = s[j][j];
+      if (!(d > 0.0) && info[p] == 0) info[p] = k0 + j + 1;
+      djj = sqrt(d);
+      s[j][j] = djj;
+    }
+    __syncthreads();
+    const double d = djj;
+    for (int i = j + 1 + threadIdx.x; i < nb; i += blockDim.x) s[i][j] = s[i][j] / d;
+    __syncthreads();
+    const int cnt = nb - j - 1;
+    for (int idx = threadIdx.x; idx < cnt * cnt; idx += blockDim.x) {
+      const int ii = idx / cnt, kk = idx - ii * cnt;
+      if (kk <= ii) s[j + 1 + ii][j + 1 + kk] = fma(-s[j + 1 + ii][j], s[j + 1 + kk][j], s[j + 1 + ii][j + 1 + kk]);
+    }
+    __syncthreads();
+  }
+  for (int idx = threadIdx.x; idx < nb * nb; idx += blockDim.x) {
+    const int r = idx / nb, c = idx - r * nb;
+    if (c <= r) A[(size_t)(k0 + r) * m + k0 + c] = s[r][c];
+  }
+}
+
+// rows below the diagonal block: x_j = (a_j - sum_{l<j} x_l L_jl) / L_jj, one thread per row
+__global__ void __launch_bounds__(64) chol_panel_kernel(double* __restrict__ Lbuf, const PulsarMeta* __restrict__ meta,
+                                                        const int* __restrict__ wide, int k0) {
+  const PulsarMeta pm = meta[wide[RG_WIDE * blockIdx.y]];
+  const int m = pm.m;
+  if (k0 + CB >= m) return;  // no rows below a full panel (a short last panel has none either)
+  double* A = Lbuf + pm.L_off;
+  __shared__ double l11[CB][CB + 1];
+  for (int idx = threadIdx.x; idx < CB * CB; idx += blockDim.x) {
+    const int r = idx / CB, c = idx - r * CB;
+    l11[r][c] = c <= r ? A[(size_t)(k0 + r) * m + k0 + c] : 0.0;
+  }
+  __syncthreads();
+  const int i = k0 + CB + blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= m) return;
+  double* Ai = A + (size_t)i * m + k0;
+  double x[CB];
+#pragma unroll
+  for (int j = 0; j < CB; ++j) {
+    double acc = Ai[j];
+#pragma unroll
+    for (int l = 0; l < j; ++l) acc = fma(-x[l], l11[j][l], acc);
+    x[j] = acc / l11[j][j];
+    Ai[j] = x[j];
+  }
+}
+
+// trailing lower triangle: a_ij -= sum_l L_il L_jl over the panel's columns, ascending; 32 x 32 tiles, 2 x 2 per thread
+__global__ void __launch_bounds__(256) chol_update_kernel(double* __restrict__ Lbuf, const PulsarMeta* __restrict__ meta,
+                                                          const int* __restrict__ wide, int k0) {
+  if (blockIdx.x > blockIdx.y) return;  // upper tiles
+  const PulsarMeta pm = meta[wide[RG_WIDE * blockIdx.z]];
+  const int m = pm.m, t0 = k0 + CB;
+  const int i0 = t0 + 32 * blockIdx.y, j0 = t0 + 32 * blockIdx.x;
+  if (i0 >= m) return;
+  double* A = Lbuf + pm.L_off;
+  __shared__ double Li[32][CB + 1], Lj[32][CB + 1];
+  for (int idx = threadIdx.x; idx < 32 * CB; idx += blockDim.x) {
+    const int r = idx / CB, c = idx - r * CB;
+    Li[r][c] = i0 + r < m ? A[(size_t)(i0 + r) * m + k0 + c] : 0.0;
+    Lj[r][c] = j0 + r < m ? A[(size_t)(j0 + r) * m + k0 + c] : 0.0;
+  }
+  __syncthreads();
+  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+#pragma unroll
+  for (int a = 0; a < 2; ++a)
+#pragma unroll
+    for (int b = 0; b < 2; ++b) {
+      const int r = ty + 16 * a, c = tx + 16 * b, i = i0 + r, j = j0 + c;
+      if (i >= m || j > i) continue;
+      double acc = A[(size_t)i * m + j];
+#pragma unroll 8
+      for (int l = 0; l < CB; ++l) acc = fma(-Li[r][l], Lj[c][l], acc);
+      A[(size_t)i * m + j] = acc;
+    }
+}
+
+// Where the G rows of one TOA of pulsar p (meta pm) live: in the pulsar's own packets, or, for a basis swept as row
+// groups (DESIGN.md section 5h), row j of group k in the packets of that group's work item at row j - r0[k]
+struct GColumn {
+  double* v[MAX_RG];  // the TOA's (t, 1/N, w, 0) in each stream (null where the stream has no such TOA)
+  double* g[MAX_RG];  // the G part of its packet
+  int il[MAX_RG], nmb[MAX_RG], r0[MAX_RG + 1];
+  int ng;
+  __device__ GColumn(double* packets, const PulsarMeta* meta, const int* wide, int n_wide, const PulsarMeta& pm, int p,
+                     int i) {
+    ng = row_groups(pm.m);
+    for (int k = 0; k < ng; ++k) {
+      const PulsarMeta& it = ng == 1 ? pm : group_meta(meta, wide, n_wide, p, k);
+      double* pk = packets + it.pk_off + (size_t)(i / it.ci) * (it.ci * (4 + it.mpad));
+      il[k] = i % it.ci;
+      v[k] = i < it.nch * it.ci ? pk + 4 * il[k] : nullptr;
+      g[k] = i < it.nch * it.ci ? pk + 4 * it.ci : nullptr;
+      nmb[k] = it.mpad >> 3;
+      r0[k] = row_group_start(pm.m, k);
+    }
+    r0[ng] = pm.m;
+  }
+  __device__ double& at(int k, int j) const { return g[k][g_frag_index(il[k], j - r0[k], nmb[k])]; }
+  // the packet stream holding row j
+  __device__ int group_of(int j) const {
+    int k = 0;
+    while (j >= r0[k + 1]) ++k;
+    return k;
+  }
+};
+
+// One thread per (padded) TOA: forward-substitute L g = T_i^T / N_i and scatter t, 1/N and g into the packet layout of
+// every stream that holds the pulsar's rows (GColumn); g is read back from the packets as the recurrence needs it,
+// so any basis width works. Padded TOAs get zeros (weight 0: they add nothing to any sum).
 __global__ void build_packets_kernel(double* __restrict__ packets,
                                      const PulsarMeta* __restrict__ meta,
                                      const double* __restrict__ Lbuf,
@@ -62,108 +206,132 @@ __global__ void build_packets_kernel(double* __restrict__ packets,
                                      const double* __restrict__ Nvec,
                                      const double* __restrict__ T,
                                      const int* __restrict__ slot_idx,
-                                     const double* __restrict__ slot_val) {
+                                     const double* __restrict__ slot_val,
+                                     const int* __restrict__ wide, int n_wide) {
   const PulsarMeta pm = meta[blockIdx.y];
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int CI = pm.ci;
-  if (i >= pm.nch * CI) return;
-  const int m = pm.m, mp = pm.mpad;
-  const int pkw = CI * (4 + mp);
-  double* pk = packets + pm.pk_off + (size_t)(i / CI) * pkw;
-  const int il = i % CI;
+  const GColumn gc(packets, meta, wide, n_wide, pm, blockIdx.y, i);
   const bool valid = i < pm.n;
   const double ninv = valid ? 1.0 / Nvec[pm.raw_off + i] : 0.0;
-  pk[4 * il] = valid ? toas[pm.raw_off + i] : 0.0;
-  pk[4 * il + 1] = ninv;
-  pk[4 * il + 2] = 0.0;  // w, filled by w_kernel
-  pk[4 * il + 3] = 0.0;
-  double* gp = pk + 4 * CI;  // G part, fragment order
-  const int nmb = mp >> 3;
-  if (!valid) {
-    for (int j = 0; j < mp; ++j) gp[g_frag_index(il, j, nmb)] = 0.0;
-    return;
+  for (int k = 0; k < gc.ng; ++k) {
+    if (!gc.v[k]) continue;
+    gc.v[k][0] = valid ? toas[pm.raw_off + i] : 0.0;
+    gc.v[k][1] = ninv;
+    gc.v[k][2] = 0.0;  // w, filled by w_kernel
+    gc.v[k][3] = 0.0;
+    // the stream's padding rows, and every row of a padded TOA
+    for (int j = valid ? gc.r0[k + 1] - gc.r0[k] : 0; j < 8 * gc.nmb[k]; ++j)
+      gc.g[k][g_frag_index(gc.il[k], j, gc.nmb[k])] = 0.0;
   }
+  if (!valid) return;
+  const int m = pm.m, mp = pm.mpad;
   const double* L = Lbuf + pm.L_off;
   const double* Ti = T + pm.T_off + (size_t)i * m;
-  double g[MAX_M];  // thread-local column of G (local memory; one-time work)
   // rows below mfix: g = L_X^-1 T_X^T / N (forward substitution); rows of the per-draw block
   // (nmfp): g = T_V^T / N - (Sigma_VX L_X^-T) g_X, i.e. the same recurrence without the division
   const int mfix = pm.mfix;
-  for (int j = 0; j < m; ++j) {
-    double acc = Ti[j] * ninv;
-    const double* Lj = L + (size_t)j * m;
-    const int kend = j < mfix ? j : mfix;
-    for (int k = 0; k < kend; ++k) acc = fma(-Lj[k], g[k], acc);
-    g[j] = j < mfix ? acc / Lj[j] : acc;
-    gp[g_frag_index(il, j, nmb)] = g[j];
-  }
-  for (int j = m; j < mp; ++j) gp[g_frag_index(il, j, nmb)] = 0.0;
+  for (int kj = 0; kj < gc.ng; ++kj)
+    for (int j = gc.r0[kj]; j < gc.r0[kj + 1]; ++j) {
+      double acc = Ti[j] * ninv;
+      const double* Lj = L + (size_t)j * m;
+      const int kend = j < mfix ? j : mfix;
+      for (int kk = 0; kk <= kj; ++kk) {
+        const int hi = gc.r0[kk + 1] < kend ? gc.r0[kk + 1] : kend;
+        for (int k = gc.r0[kk]; k < hi; ++k) acc = fma(-Lj[k], gc.at(kk, k), acc);
+      }
+      gc.at(kj, j) = j < mfix ? acc / Lj[j] : acc;
+    }
   // block-diagonal N: the last row block holds the epoch slots; this TOA feeds sqrt(beta_e)/N_i
   // into the slot of its epoch (fp_sweep_kernel folds the slot sums when the epoch ends)
   if (slot_idx != nullptr) {
     const int sidx = slot_idx[pm.raw_off + i];
-    if (sidx >= 0) gp[g_frag_index(il, mp - 8 + sidx, nmb)] = slot_val[pm.raw_off + i];
+    if (sidx >= 0) gc.g[0][g_frag_index(gc.il[0], mp - 8 + sidx, gc.nmb[0])] = slot_val[pm.raw_off + i];
   }
 }
 
 // u_r[j] = sum_i G[j][i] r_i. One CTA per pulsar, one warp per basis row at a time; lanes
 // stride over TOAs, fixed-order shuffle tree: deterministic.
 __global__ void ur_kernel(const double* __restrict__ packets, const PulsarMeta* __restrict__ meta,
-                          const double* __restrict__ res, double* __restrict__ ur) {
+                          const double* __restrict__ res, double* __restrict__ ur, int ld, const int* __restrict__ wide,
+                          int n_wide) {
   const PulsarMeta pm = meta[blockIdx.x];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  const int CI = pm.ci;
-  const int mp = pm.mpad, pkw = CI * (4 + mp);
-  const double* pk0 = packets + pm.pk_off;
   for (int j = wid; j < pm.m; j += nw) {
+    // the stream holding row j: the pulsar's own packets or those of its row group
+    int k = 0;
+    while (j >= row_group_start(pm.m, k + 1)) ++k;
+    const PulsarMeta& it = row_groups(pm.m) == 1 ? pm : group_meta(meta, wide, n_wide, blockIdx.x, k);
+    const int jl = j - row_group_start(pm.m, k);
+    const int CI = it.ci, mp = it.mpad, pkw = CI * (4 + mp);
+    const double* pk0 = packets + it.pk_off;
     double acc = 0.0;
     for (int i = lane; i < pm.n; i += 32) {
-      const double g = pk0[(size_t)(i / CI) * pkw + 4 * CI + g_frag_index(i % CI, j, mp >> 3)];
+      const double g = pk0[(size_t)(i / CI) * pkw + 4 * CI + g_frag_index(i % CI, jl, mp >> 3)];
       acc = fma(g, res[pm.raw_off + i], acc);
     }
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-    if (lane == 0) ur[(size_t)blockIdx.x * MAX_M + j] = acc;
+    if (lane == 0) ur[(size_t)blockIdx.x * ld + j] = acc;
   }
 }
 
-// w_i = r_i / N_i - sum_{j < mfix} G[j][i] u_r[j]   (= (C^-1 r)_i for a plain-Fp pack)
+// w_i = r_i / N_i - sum_{j < mfix} G[j][i] u_r[j], rows in order 0 .. mfix-1 across the row groups (= (C^-1 r)_i for a
+// plain-Fp pack), into the vector part of every stream that holds the pulsar's rows
 __global__ void w_kernel(double* __restrict__ packets, const PulsarMeta* __restrict__ meta,
-                         const double* __restrict__ res, const double* __restrict__ ur) {
+                         const double* __restrict__ res, const double* __restrict__ ur, int ld,
+                         const int* __restrict__ wide, int n_wide) {
   const PulsarMeta pm = meta[blockIdx.y];
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= pm.n) return;
-  const int CI = pm.ci;
-  const int mp = pm.mpad, pkw = CI * (4 + mp);
-  double* pk = packets + pm.pk_off + (size_t)(i / CI) * pkw;
-  const int il = i % CI;
-  const double* gp = pk + 4 * CI;
-  const double* u = ur + (size_t)blockIdx.y * MAX_M;
+  const GColumn gc(packets, meta, wide, n_wide, pm, blockIdx.y, i);
+  const double* u = ur + (size_t)blockIdx.y * ld;
   double acc = 0.0;
-  for (int j = 0; j < pm.mfix; ++j) acc = fma(gp[g_frag_index(il, j, mp >> 3)], u[j], acc);
-  pk[4 * il + 2] = res[pm.raw_off + i] * pk[4 * il + 1] - acc;
+  for (int k = 0; k < gc.ng; ++k) {
+    const int hi = gc.r0[k + 1] < pm.mfix ? gc.r0[k + 1] : pm.mfix;
+    for (int j = gc.r0[k]; j < hi; ++j) acc = fma(gc.at(k, j), u[j], acc);
+  }
+  for (int k = 0; k < gc.ng; ++k) gc.v[k][2] = res[pm.raw_off + i] * gc.v[k][1] - acc;
 }
 
 int launch_fp_precompute(fastfp_pack* pk, const double* d_toas, const double* d_res,
                          const double* d_Nvec, const double* d_T, cudaStream_t st, double* d_ur_keep,
                          const BlockNDev* bn) {
   const int P = pk->P;
-  int nmax = 0;
-  for (auto& m : pk->meta) nmax = m.nch * m.ci > nmax ? m.nch * m.ci : nmax;
+  int nmax = 0, ld = MAX_M;  // ld: row length of u_r (d_ur_keep: nmfp packs, m <= MAX_M)
+  for (auto& m : pk->meta) {
+    nmax = m.nch * m.ci > nmax ? m.nch * m.ci : nmax;
+    ld = m.m > ld ? m.m : ld;
+  }
+  for (auto& m : pk->items) nmax = m.nch * m.ci > nmax ? m.nch * m.ci : nmax;
   DeviceBuf<double> ur_tmp;
   double* d_ur = d_ur_keep;
   if (!d_ur) {
-    FFP_CUDA(dev_alloc(&ur_tmp, (size_t)P * MAX_M));
+    FFP_CUDA(dev_alloc(&ur_tmp, (size_t)P * ld));
     d_ur = ur_tmp.get();
   }
   const PackCore& c = pk->core;
   chol_kernel<<<P, 256, 0, st>>>(c.L.get(), c.meta.get(), c.info.get());
+  g_launches += 1;
+  int mwide = 0;
+  for (auto& m : pk->meta) mwide = row_groups(m.m) > 1 && m.m > mwide ? m.m : mwide;
+  for (int k0 = 0; k0 < mwide; k0 += CB) {
+    chol_diag_kernel<<<pk->n_wide, 256, 0, st>>>(c.L.get(), c.meta.get(), c.info.get(), c.wide.get(), k0);
+    g_launches += 1;
+    const int below = mwide - k0 - CB;
+    if (below <= 0) continue;
+    chol_panel_kernel<<<dim3((below + 63) / 64, pk->n_wide), 64, 0, st>>>(c.L.get(), c.meta.get(), c.wide.get(), k0);
+    const int nt = (below + 31) / 32;
+    chol_update_kernel<<<dim3(nt, nt, pk->n_wide), 256, 0, st>>>(c.L.get(), c.meta.get(), c.wide.get(), k0);
+    g_launches += 2;
+  }
   dim3 g1((nmax + 127) / 128, P);
   build_packets_kernel<<<g1, 128, 0, st>>>(c.packets.get(), c.meta.get(), c.L.get(), d_toas, d_Nvec, d_T,
-                                           bn ? bn->slot_idx : nullptr, bn ? bn->slot_val : nullptr);
-  ur_kernel<<<P, 256, 0, st>>>(c.packets.get(), c.meta.get(), d_res, d_ur);
+                                           bn ? bn->slot_idx : nullptr, bn ? bn->slot_val : nullptr, c.wide.get(),
+                                           pk->n_wide);
+  ur_kernel<<<P, 256, 0, st>>>(c.packets.get(), c.meta.get(), d_res, d_ur, ld, c.wide.get(), pk->n_wide);
   // with a block-diagonal N the first term of w is N^-1 r, supplied as (N^-1 r) * Nvec
-  w_kernel<<<g1, 128, 0, st>>>(c.packets.get(), c.meta.get(), bn ? bn->res_w : d_res, d_ur);
-  g_launches += 4;
+  w_kernel<<<g1, 128, 0, st>>>(c.packets.get(), c.meta.get(), bn ? bn->res_w : d_res, d_ur, ld, c.wide.get(),
+                               pk->n_wide);
+  g_launches += 3;
   FFP_CUDA(cudaGetLastError());
   FFP_CUDA(cudaStreamSynchronize(st));
   // the factorisation status comes back with the pack: a non-positive pivot means Sigma was not numerically

@@ -67,6 +67,14 @@ int fastfp_pack_create(int device, int P, const int64_t* n, const int64_t* m,
                        const double* const* Nvecs, const double* const* Ts,
                        const double* const* sigmas, void* stream, fastfp_pack_t** out);
 
+/* Basis width: m_p <= 2688 columns. One work item of the sweep kernel holds up to 640 G rows; a wider basis is swept
+ * as row groups, each one work item, whose b-sums a combine step adds (DESIGN.md section 5h). Above 2688,
+ * fastfp_pack_create returns FASTFP_ERR_UNSUPPORTED. Block-diagonal-N packs (m_p <= 632), noise-marginalised packs
+ * (m_p <= 640) and residual batches (every m_p <= 640) keep the width of one work item.
+ * fastfp_row_groups: the row groups of a basis of width m: their number g (0 if m is outside 1 .. 2688), and with
+ * starts non-NULL the first row of each group, starts[0..g] (starts[g] = m). g == 1 for m <= 640. */
+int fastfp_row_groups(int64_t m, int64_t* starts);
+
 /* fastfp_fp_sweep: jax.vmap(FastFp.calculate_Fp, in_axes=(0,None,None,None))(freqs, ...)
  * (examples/run_fp.py:63-64; per-frequency body fastfp/fastfp.py:69-92).  out[f] = Fp(freqs[f]),
  * the pulsar sum taken in pulsar order starting from 0 (fastfp.py:71,90). */
